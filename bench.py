@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- decode tokens/s at batch 1 on B200 (BASELINE.json metric), plus roofline, parity and CPU baseline.
+"""bench.py -- decode tokens/s at batch 1 on H100 (BASELINE.json metric), plus roofline, parity and CPU baseline.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload nano-168m-q80|qwen3-0.6b-q80|qwen3-0.6b-q4k|...]
+                    [--dump-outputs DIR]
     python bench.py --impl reference ...        # the reference's own OpenMP CPU engine on the host cores
 
 A *step* is one pass of the hot path over one batch of synthetic input: a 16-token prompt is pushed through the
@@ -24,6 +25,10 @@ token-at-a-time path (infer.c:1258-1260), then greedy decode (temperature 0, rep
   cpu_baseline : the unmodified reference (oracle/_ref, Makefile flags) on the host cores over a bounded sample.
 
 N > 1 (torchrun): `value` = N independent batch-1 sessions (the path shards by session: no data-path collective => "weak").
+
+--dump-outputs DIR: after the timed steps, what the last one computed is written as DIR/ids.npy (the token ids the device loop
+returned, prompt included, float64) and DIR/logits.npy (the logits of the last decoded position, float32).  The model files and
+prompts are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -74,12 +79,12 @@ BPW = {mf.QUANT_F32: lambda gs: 4.0, mf.QUANT_Q80: lambda gs: 1.0 + 4.0 / max(gs
 
 
 def workload_config(name):
-    """The `config` object: identical in the B200 arm and in the reference arm."""
+    """The `config` object: identical in the GPU arm and in the reference arm."""
     preset, quant, gs, seq = WORKLOADS[name]
     spec = mf.PRESETS[preset]
     wbytes = spec.n_weights() * BPW[quant](gs)
     return {"workload": f"{name} greedy decode, seq={seq}, prompt={PROMPT}, max_seq_len={seq}",
-            "l2": "inputs larger than L2: %.0f MB of weights (+ the KV cache) are streamed per token vs 126 MB of L2" % (wbytes / 1e6),
+            "l2": "inputs larger than L2: %.0f MB of weights (+ the KV cache) are streamed per token vs 50 MB of L2" % (wbytes / 1e6),
             "timing": "decode segment of each step (tokens %d..%d); GPU: CUDA events on the launching stream, max over ranks; CPU: wall clock" % (PROMPT, seq - 1)}
 
 
@@ -101,11 +106,11 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons sampled during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -220,7 +225,7 @@ def cpu_sweep(path, spec, seq, budget_s=30.0):
 
 
 def cpu_baseline(workload, path, spec, seq, runs=1):
-    """`cpu_baseline` of the B200 arm: thread sweep on a probe, then the bounded sample (prompt + 64 decode positions) at the best setting."""
+    """`cpu_baseline` of the GPU arm: thread sweep on a probe, then the bounded sample (prompt + 64 decode positions) at the best setting."""
     kind, flavour, best, table, ncpu, _ = cpu_sweep(path, spec, seq, budget_s=20.0)
     if best is None:
         return {"value": None, "unit": "tokens/s", "cores": 0, "kind": kind, "sample": "failed"}
@@ -352,6 +357,7 @@ def measure(E, workload, steps, warmup, local, dist=None, world=1, flags=0, e2e=
     res = {"value": value, "ms_per_step": wall * 1e3 / steps, "gpu_launches": int(launches), "launches_per_token": eng.launches_per_token,
            "engine": eng.path, "path_calibration": eng.calibration, "dec_ms": dec_ms}
     timed_ids = ids.copy()
+    res["outputs"] = {"ids": timed_ids[:seq].astype(np.float64), "logits": eng.logits()}     # before anything else runs on the engine
 
     if e2e:
         e2e_steps = max(1, min(steps, 2))
@@ -394,17 +400,10 @@ def measure(E, workload, steps, warmup, local, dist=None, world=1, flags=0, e2e=
             if cnt[i]:
                 dur = float(ms[i]) / int(cnt[i]) * 1e-3
                 per_class[name] = {"launches": int(cnt[i]), "mean_us": dur * 1e6, "share": float(ms[i]) / tot_ms, "alg_bytes": alg[name], "gbs": alg[name] / dur / 1e9}
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json"))).get(workload + (":stream" if eng.path.startswith("streaming") else ":multikernel"))
-    except Exception:
-        pass
     if eng.path.startswith("streaming"):
         # the step IS one kernel: a launch decodes n_dec tokens, so the dominant kernel's roofline is the token roofline
         res["roofline"] = {"bound": "hbm", "kernel": f"k_decode_stream (one launch decodes {n_dec} tokens: all layers + classifier + argmax)",
                            "achieved": per_gpu_gbs, "peak": peak, "unit": "GB/s", "frac": per_gpu_gbs / peak,
-                           "traffic": traffic * n_dec if traffic else None,
-                           "traffic_source": f"ncu --set full capture of one k_decode_stream launch: DRAM bytes per token x {n_dec} tokens (profiles/r2_ncu_stream.md)" if traffic else None,
                            "peak_source": peak_src, "alg_bytes_per_launch": bytes_tok * n_dec, "mean_launch_us": dec_ms / steps * 1e3, "share_of_step": 1.0,
                            "phase_profile_note": "per_kernel = the multi-kernel path's kernels for the same phases (graph/PDL off, CUDA events per launch), for orientation only",
                            "per_kernel": per_class}
@@ -412,7 +411,6 @@ def measure(E, workload, steps, warmup, local, dist=None, world=1, flags=0, e2e=
         dom = "w13_swiglu"
         res["roofline"] = {"bound": "hbm", "kernel": f"k_matvec<{'Q80' if quant == mf.QUANT_Q80 else 'Q4K' if quant == mf.QUANT_Q4K else 'F32'},SWIGLU> (W1|W3 + SwiGLU)",
                            "achieved": per_class[dom]["gbs"], "peak": peak, "unit": "GB/s", "frac": per_class[dom]["gbs"] / peak,
-                           "traffic": traffic, "traffic_source": "ncu --set full capture (profiles/r2_ncu_multikernel.md)" if traffic else None,
                            "peak_source": peak_src, "alg_bytes_per_launch": per_class[dom]["alg_bytes"], "mean_launch_us": per_class[dom]["mean_us"],
                            "share_of_step": per_class[dom]["share"], "per_kernel": per_class}
     if parity:
@@ -487,7 +485,7 @@ def main():
     ap.add_argument("--workload", default="nano-168m-q80", choices=sorted(WORKLOADS))
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--mode", default="replicas", choices=["replicas", "tp"],
-                    help="replicas: one independent batch-1 session per GPU (weak scaling, the default the driver runs; a `tp` block is added for N > 1); "
+                    help="replicas: one independent batch-1 session per GPU (weak scaling, the default; a `tp` block is added for N > 1); "
                          "tp: only the tensor-parallel block (ONE session sharded over the GPUs)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra configs / exact-mode / tp blocks (quick runs)")
@@ -495,7 +493,10 @@ def main():
     ap.add_argument("--no-pdl", action="store_true")
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-stream", action="store_true", help="forbid the streaming kernel")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's ids and logits as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.mode == "tp"):
+        ap.error("--dump-outputs writes what the GPU replicas path computed; it is not available with --impl reference or --mode tp")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
     preset, quant, gs, seq = WORKLOADS[args.workload]
@@ -527,6 +528,11 @@ def main():
         sampler.start()
     res = measure(E, args.workload, args.steps, args.warmup, local, dist, world, flags, parity=(rank == 0))
     clocks = sampler.stop() if rank == 0 else None
+    outputs = res.pop("outputs")
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in outputs.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
 
     tp = None
     if world > 1 and not args.no_extra:

@@ -1,5 +1,5 @@
 /*
- * nano_b200.h -- C-ABI of the B200 (sm_100a) batch-1 decode engine for bd4sur/Nano model files.
+ * nano_b200.h -- C-ABI of the H100 (sm_90a) batch-1 decode engine for bd4sur/Nano model files.
  *
  * This is the "thin C-ABI" under the reference's own host API (infer/infer.h, infer/tensor.h): the
  * reference-facing shim (include/nano_infer_abi.h, nano_b200/csrc/infer_b200.c) implements

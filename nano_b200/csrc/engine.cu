@@ -553,8 +553,9 @@ int setup_stream(nb200_engine *e) {
         T -= T % sk.unit_rows;
         if (T > max_rows) T = max_rows;
         if (T < sk.unit_rows) return 0;
-        // many rows per CTA: throughput mode, every tile is consumed by one warp -- small tiles so that all 15 warps have one
-        sk.owned = (max_rows >= env_u32("NB200_OWNED_ROWS", 32) || (uint64_t)max_rows * rowb >= (uint64_t)env_u32("NB200_OWNED_KB", 32) * 1024u) ? 1u : 0u;
+        // many rows per CTA: throughput mode, every tile is consumed by one warp -- small tiles so that all 15 warps have one.
+        // 64 rows: measured on H100 against 16 / 32 (Nano-168M Q80 1519 vs 1473 / 1443 tok/s, Qwen3-0.6B Q4K 892 vs 879 / 886)
+        sk.owned = (max_rows >= env_u32("NB200_OWNED_ROWS", 64) || (uint64_t)max_rows * rowb >= (uint64_t)env_u32("NB200_OWNED_KB", 32) * 1024u) ? 1u : 0u;
         if (sk.owned) {
             uint32_t t2 = (max_rows + kConsWarps - 1) / kConsWarps;
             t2 = ((t2 + sk.unit_rows - 1) / sk.unit_rows) * sk.unit_rows;
@@ -925,7 +926,7 @@ static int create_impl(nb200_engine **out, const uint8_t *img, uint64_t image_by
     {
         // Default path in fast mode on one GPU.  The streaming kernel is set up whenever the shape allows it.  F32 / Q4K models and Q80
         // models under 256 MB of weights always run it (latency-bound: one launch, no kernel boundary per phase).  For larger Q80 models
-        // neither path wins everywhere (profiles/r2_paths.md: multi-kernel ahead at 0.6B / 1.7B, streaming ahead at 4B with a long context),
+        // neither path wins everywhere (on one H100 the multi-kernel path is ahead for Qwen3-0.6B @2048, DESIGN.md section 5.2),
         // so the engine times both at the middle of its context and keeps the faster one (calibrate_paths).
         // NB200_STREAM=1 forces the streaming kernel where the shape allows it, NB200_STREAM=0 / NB200_FLAG_NO_STREAM forbid it.
         const char *st_env = getenv("NB200_STREAM");

@@ -1,4 +1,4 @@
-// kernels.cuh -- sm_100a device code of the batch-1 decode engine.
+// kernels.cuh -- sm_90a device code of the batch-1 decode engine.
 //
 // Everything on the per-token path of the reference (infer/infer.c:584-1018, infer/tensor.c) is here:
 //   activation prep ....... rmsnorm (infer.c:601) + Q80 quantize (tensor.c:21) / Q4K quantize (tensor.c:144)

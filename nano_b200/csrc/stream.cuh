@@ -12,9 +12,9 @@
 // L2-resident vectors of 64-bit words {fp32 value, 32-bit epoch}: a producing warp publishes a finished element with
 // ONE 8-byte store, a consuming CTA polls the words it needs until they carry the epoch of the exchange it is waiting
 // for.  Value and epoch arrive together (single-copy atomic), so there is no fence, no counter and no grid barrier on
-// the per-phase path (measured on B200: release fence ~1.1-1.7 k cycles, counter barrier ~1.6 k, against ~0.3-0.6 k
-// for a store -> poll hand-off).  Vectors that every CTA reads are written to kStRep replicas (different L2 slices;
-// one hot copy read by 148 SMs at once costs ~600 cycles of slice bandwidth).
+// the per-phase path (a release fence or a counter barrier costs several times a store -> poll hand-off: tools/micro/
+// lat_bench.cu, bar_bench.cu).  Vectors that every CTA reads are written to kStRep replicas (different L2 slices, so
+// that all SMs reading one hot copy at once do not queue on one slice: tools/micro/exchange_bench.cu).
 //   Why a word is never overwritten before its readers are done: a CTA reads an entire vector before it produces
 //   anything of the next exchange, so "all of exchange k has arrived" implies every producer of exchange k has finished
 //   reading exchange k-1; the writer of a later exchange into the same buffer has (transitively) seen all of k.

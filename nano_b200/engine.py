@@ -112,7 +112,7 @@ def _p(a: np.ndarray, t):
 
 
 class Engine:
-    """One model resident in the HBM of one B200."""
+    """One model resident in the HBM of one GPU."""
 
     def __init__(self, model, max_seq: int, device: int = 0, flags: int = 0, tp: Optional[Tuple[int, int]] = None):
         """tp=(rank, size) creates one rank of a tensor-parallel group; attach it (tp_attach_ipc / TpGroup) before use."""

@@ -22,6 +22,8 @@ os.environ.setdefault("OMP_WAIT_POLICY", "passive")
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REF_DIR = os.path.join(HERE, "_ref")
+REFHOST_SO = os.path.join(REF_DIR, "libnano_refhost.so")     # the reference's tokenizer / utils / HAL objects the shim imports
+NANO_CLI = os.path.join(REF_DIR, "nano_cli")
 REFERENCE_SRC = "/root/reference/infer"
 
 f32p = C.POINTER(C.c_float)

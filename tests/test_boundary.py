@@ -62,9 +62,9 @@ def test_shim_exports_reference_api():
     assert "nb200_engine_create" in und and "oracle" not in subprocess.run(["ldd", nb_build.SHIM_SO], capture_output=True, text=True).stdout
 
 
-@pytest.mark.skipif(not nb_build.reference_present(), reason="/root/reference not present on this box")
+@pytest.mark.skipif(not os.path.exists(ob.NANO_CLI), reason="nano_cli not linked (needs the reference tree at build time)")
 def test_reference_nano_cli_links_unchanged():
-    exe = nb_build.build_nano_cli(force=True)
+    exe = ob.NANO_CLI
     und = subprocess.run(["nm", "-D", "--undefined-only", exe], capture_output=True, text=True, check=True).stdout
     assert " U llm_context_init" in und and " U generate_sync" in und
     ldd = subprocess.run(["ldd", exe], capture_output=True, text=True).stdout

@@ -33,9 +33,9 @@ def test_binding_covers_header():
         assert hasattr(L, s)
 
 
-def test_sm100a_code_is_embedded():
+def test_sm90a_code_is_embedded():
     out = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-lelf", nb_build.ENGINE_SO], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 @pytest.mark.skipif(E.device_count() > 0, reason="box has a GPU")

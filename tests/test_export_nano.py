@@ -1,66 +1,51 @@
-"""CPU test of the Nano checkpoint export (nano_b200/export_nano.py; SURVEY section 8 row f1): a small randomly initialised instance of the
-reference's own PyTorch model (model.py, imported from /root/reference in this container only) is exported by OUR exporter and by the
-reference's export.py -- the two files must be byte-identical (F32 and Q80) -- and the file's logits (oracle) must equal the PyTorch
-model's forward pass."""
-import importlib.util
+"""CPU test of the Nano checkpoint export (nano_b200/export_nano.py; SURVEY section 8 row f1).  A seeded tiny GPT in the reference's
+module naming (tests/golden/make_golden.py:nano_export_weights) is exported by OUR exporter; the files must be byte-identical to what
+the reference's own export.py wrote for the same weights (F32, Q80 and a LoRA plug-in; SHA-256 digests in tests/golden/export_nano.npz),
+and the F32 file's logits (oracle) must equal the reference PyTorch model's forward pass stored beside them."""
 import os
 import sys
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
 torch = pytest.importorskip("torch")
 
-from nano_b200 import export_nano, modelfile as mf
-from oracle import bindings as ob
+from conftest import GOLDEN  # noqa: E402
+from nano_b200 import export_nano, modelfile as mf  # noqa: E402
+from oracle import bindings as ob  # noqa: E402
 
-REF = os.environ.get("NANO_REFERENCE_ROOT", "/root/reference")
-pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(REF, "model.py")), reason="the reference tree is not present")
-S = 12
+sys.path.insert(0, GOLDEN)
+from make_golden import NANO_EXPORT_CONFIG, NANO_EXPORT_LORA, NANO_EXPORT_SEQ, nano_export_tokenizer, nano_export_weights, sha  # noqa: E402
+sys.path.remove(GOLDEN)
 
-
-@pytest.fixture(scope="module")
-def ref_modules():
-    sys.path.insert(0, REF)
-    try:
-        import model as ref_model                    # the reference's model.py
-        spec = importlib.util.spec_from_file_location("nano_ref_export", os.path.join(REF, "export.py"))
-        ref_export = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(ref_export)
-    finally:
-        sys.path.remove(REF)
-    return ref_model, ref_export
+S = NANO_EXPORT_SEQ
+GOLD = np.load(os.path.join(GOLDEN, "export_nano.npz"))
 
 
-def tiny_gpt(ref_model, seed=5):
-    torch.manual_seed(seed)
-    cfg = ref_model.ModelConfig(block_size=32, vocab_size=160, n_layer=2, n_embd=128, n_head=4, n_kv_head=2, n_hidden=256)
-    m = ref_model.GPT(cfg).float().eval()
-    with torch.no_grad():
-        for n, p in m.named_parameters():
-            if "norm" in n:
-                p.add_(0.1 * torch.randn_like(p))
-            else:
-                p.mul_(3.0)
-    return m
+class TinyGPT:
+    """What export_nano reads from a checkpoint's model: .config, .state_dict() (tied classifier: one tensor under both names)
+    and the RoPE tables the model carries."""
+
+    def __init__(self, sd):
+        self.config = SimpleNamespace(**NANO_EXPORT_CONFIG)
+        self._sd = {k: torch.from_numpy(v) for k, v in sd.items() if k != "output.weight"}
+        self._sd["output.weight"] = self._sd["tok_embeddings.weight"]
+        self.freqs_cos, self.freqs_sin = torch.from_numpy(GOLD["freqs_cos"]), torch.from_numpy(GOLD["freqs_sin"])
+
+    def state_dict(self):
+        return self._sd
 
 
-def test_export_is_byte_identical_to_the_reference_exporter_and_matches_the_model(tmp_path, ref_modules, capsys):
-    ref_model, ref_export = ref_modules
-    m = tiny_gpt(ref_model)
-    V = m.config.vocab_size
-    tok = {"itos": [chr(0x4E00 + i) for i in range(V)], "vocab_size": V, "special_tokens": [chr(0x4E00), chr(0x4E01)]}
-    toks = mf.teacher_tokens(S, V)
-    with torch.no_grad():
-        want = np.stack([m(torch.tensor([list(map(int, toks[: p + 1]))], dtype=torch.long))[0][0, -1].float().numpy() for p in range(S)])
+def test_export_is_byte_identical_to_the_reference_exporter_and_matches_the_model(tmp_path):
+    sd, _lora = nano_export_weights()
+    m = TinyGPT(sd)
+    ours = str(tmp_path / "ours.bin")
+    export_nano.export_nano(m, ours, mf.QUANT_F32, tokenizer_config=nano_export_tokenizer())
+    assert sha(open(ours, "rb").read()) == str(GOLD["f32_sha256"]), "F32 export differs from the reference exporter's file"
 
-    ours, theirs = str(tmp_path / "ours.bin"), str(tmp_path / "theirs.bin")
-    export_nano.export_nano(m, ours, mf.QUANT_F32, tokenizer_config=tok)
-    ref_export.export_model(m, tok, theirs)
-    a, b = open(ours, "rb").read(), open(theirs, "rb").read()
-    assert len(a) == len(b), (len(a), len(b))
-    assert a == b, "F32 export differs from the reference exporter at byte %d" % next(i for i in range(len(a)) if a[i] != b[i])
-
+    want = GOLD["logits"]                                                          # the reference PyTorch model, positions 0..S-1
+    toks = mf.teacher_tokens(S, NANO_EXPORT_CONFIG["vocab_size"])
     o = ob.NanoOracle(ours, S)
     got = np.stack([o.forward(int(toks[p]), p) for p in range(S)])
     o.close()
@@ -68,45 +53,19 @@ def test_export_is_byte_identical_to_the_reference_exporter_and_matches_the_mode
     print(f"exported F32 file vs the PyTorch model: max|dlogit| {err:.3e} (logit scale {scale:.2f})")
     assert err < 2e-4 * max(1.0, scale)
 
-    oursq, theirsq = str(tmp_path / "ours_q80.bin"), str(tmp_path / "theirs_q80.bin")
-    export_nano.export_nano(m, oursq, mf.QUANT_Q80, 64, tokenizer_config=tok)
-    ref_export.export_quantized(m, tok, theirsq, group_size=64)
-    a, b = open(oursq, "rb").read(), open(theirsq, "rb").read()
-    assert len(a) == len(b), (len(a), len(b))
-    assert a == b, "Q80 export differs from the reference exporter at byte %d" % next(i for i in range(len(a)) if a[i] != b[i])
+    oursq = str(tmp_path / "ours_q80.bin")
+    export_nano.export_nano(m, oursq, mf.QUANT_Q80, 64, tokenizer_config=nano_export_tokenizer())
+    assert sha(open(oursq, "rb").read()) == str(GOLD["q80_sha256"]), "Q80 export differs from the reference exporter's file"
 
 
-def test_lora_export_is_byte_identical_and_the_reference_engine_reproduces_the_lora_model(tmp_path, ref_modules):
-    """export.py:117-226 / infer.c:436-500 and the LoRA branches infer.c:792-808, :898-903: base file + plug-in run by the unmodified
-    reference engine against the PyTorch model with the same low-rank branches attached."""
-    ref_model, ref_export = ref_modules
-    m = tiny_gpt(ref_model, seed=9)
-    V = m.config.vocab_size
-    tok = {"itos": [chr(0x4E00 + i) for i in range(V)], "vocab_size": V, "special_tokens": []}
-    base = str(tmp_path / "base.bin")
-    export_nano.export_nano(m, base, mf.QUANT_F32, tokenizer_config=tok)           # the base model, before the branches are attached
-    m.to_lora(lora_rank=4, lora_alpha=8)
-    torch.manual_seed(11)
-    with torch.no_grad():
-        for n, p in m.named_parameters():
-            if "lora_b" in n:
-                p.copy_(0.05 * torch.randn_like(p))                                  # B starts at zero: make the branch contribute
-    m.eval()
-    lora_sd = m.get_lora_state_dict()
-    ours, theirs = str(tmp_path / "lora_ours.bin"), str(tmp_path / "lora_theirs.bin")
-    export_nano.export_lora(lora_sd, 4, 8, m.config, ours)
-    ref_export.export_lora(lora_sd, {"lora_rank": 4, "lora_alpha": 8}, m.config, theirs)
-    a, b = open(ours, "rb").read(), open(theirs, "rb").read()
-    assert a == b, "LoRA export differs from the reference exporter"
-    if not ob.ref_available("strict"):
-        pytest.skip("oracle/_ref not built: byte identity checked only")
-    toks = mf.teacher_tokens(S, V)
-    with torch.no_grad():
-        want = np.stack([m(torch.tensor([list(map(int, toks[: p + 1]))], dtype=torch.long))[0][0, -1].float().numpy() for p in range(S)])
-    r = ob.RefEngine(base, S)
-    r.load_lora(a)
-    got = np.stack([r.forward(int(toks[p]), p) for p in range(S)])
-    r.close()
-    err, scale = float(np.abs(got - want).max()), float(np.abs(want).max())
-    print(f"reference engine (base file + exported plug-in) vs the PyTorch LoRA model: max|dlogit| {err:.3e} (logit scale {scale:.2f})")
-    assert err < 2e-4 * max(1.0, scale)
+def test_lora_export_is_byte_identical_and_the_reference_engine_reproduces_the_lora_model(tmp_path):
+    """export.py:117-226 / infer.c:436-500: the plug-in file is byte-identical to the reference exporter's for the same LoRA
+    state dict, so the reference engine (and this engine, tests/test_gpu_lora.py) reads exactly the branches the model has."""
+    _sd, lora = nano_export_weights()
+    rank, alpha = NANO_EXPORT_LORA
+    ours = str(tmp_path / "lora_ours.bin")
+    info = export_nano.export_lora({k: torch.from_numpy(v) for k, v in lora.items()}, rank, alpha, SimpleNamespace(**NANO_EXPORT_CONFIG), ours)
+    c = NANO_EXPORT_CONFIG
+    kv = c["n_kv_head"] * c["n_embd"] // c["n_head"]
+    assert info["bytes"] == 256 + 4 * c["n_layer"] * rank * (4 * c["n_embd"] + 2 * c["n_embd"] + 2 * kv)
+    assert sha(open(ours, "rb").read()) == str(GOLD["lora_sha256"]), "LoRA export differs from the reference exporter's file"

@@ -16,7 +16,7 @@ from oracle import bindings as ob
 
 pytestmark = pytest.mark.gpu
 
-HAVE_REFHOST = os.path.exists(nb_build.REFHOST_SO)
+HAVE_REFHOST = os.path.exists(ob.REFHOST_SO)
 needs_refhost = pytest.mark.skipif(not HAVE_REFHOST, reason="libnano_refhost.so (reference tokenizer/utils objects) not built")
 
 
@@ -32,7 +32,7 @@ _shim = None
 def shim():
     global _shim
     if _shim is None:
-        C.CDLL(nb_build.REFHOST_SO, mode=C.RTLD_GLOBAL)        # the reference's own tokenizer.c/utils.c/hal objects
+        C.CDLL(ob.REFHOST_SO, mode=C.RTLD_GLOBAL)        # the reference's own tokenizer.c/utils.c/hal objects
         L = C.CDLL(nb_build.SHIM_SO, mode=C.RTLD_GLOBAL)
         L.llm_context_init.restype = C.c_void_p
         L.llm_context_init.argtypes = [C.c_char_p, C.c_char_p, C.c_uint32, C.c_float, C.c_float, C.c_float, C.c_uint32, C.c_uint64]
@@ -135,15 +135,16 @@ def test_session_api_runs_and_stops_at_length():
     L.llm_context_free(ctx)
 
 
-@pytest.mark.skipif(not os.path.exists(nb_build.NANO_CLI), reason="nano_cli not linked on this box")
+@pytest.mark.skipif(not os.path.exists(ob.NANO_CLI), reason="nano_cli not linked (needs the reference tree at build time)")
 def test_nano_cli_binary_starts_and_reports_missing_model():
     """The unmodified main_cli.c linked against our libraries runs; its model path is hard-coded (main_cli.c:12),
     so without that file it must exit through the reference's own error path."""
-    r = subprocess.run([nb_build.NANO_CLI], input=b"", capture_output=True, timeout=60)
+    r = subprocess.run([ob.NANO_CLI], input=b"", capture_output=True, timeout=60)
     assert r.returncode != 0
     assert b"open" in r.stderr.lower() or b"couldn" in r.stderr.lower()
 
 
+@needs_refhost
 def test_q4k_tensor_functions_through_reference_names():
     """tensor.h:160-166 as the reference's tools/export_q4k.c calls them (quantize_tensor_q4k -> matmul_q4k on a 3-D
     weight with a layer index), against the outputs committed from the unmodified reference and the oracle."""

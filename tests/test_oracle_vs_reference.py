@@ -1,11 +1,12 @@
 """CPU tests: pin the oracle (oracle/nano_oracle.c) to the reference and to the committed goldens.
 
 The reference has no test suite (SURVEY section 4); what pins behaviour is the embedded sort model
-(infer/main_sort.c:6-3098, README.md:379) plus outputs of the reference compiled here.
+(infer/main_sort.c:6-3098, README.md:379) plus outputs of the unmodified strict reference, stored under tests/golden/
+(SHA-256 digests in reference_outputs.json where the comparison is bit-exact; tests/golden/make_golden.py regenerates them).
 """
-import ctypes as C
 import json
 import os
+import sys
 
 import numpy as np
 import pytest
@@ -14,8 +15,12 @@ from conftest import GOLDEN, assert_bits_equal
 from nano_b200 import modelfile as mf
 from oracle import bindings as ob
 
-HAVE_REF = ob.ref_available("strict")
-needs_ref = pytest.mark.skipif(not HAVE_REF, reason="oracle/_ref not built (no /root/reference here)")
+sys.path.insert(0, GOLDEN)
+from make_golden import (LORA_CASES, STRICT_CASES, STRICT_SEQ, TOY_POSITIONS, q4k_writer_input,  # noqa: E402
+                         q80_ops_inputs, sha)
+sys.path.remove(GOLDEN)
+
+REF_OUT = json.load(open(os.path.join(GOLDEN, "reference_outputs.json")))
 
 TOY = [("toy-nano", mf.QUANT_F32, 128), ("toy-nano", mf.QUANT_Q80, 64), ("toy-nano", mf.QUANT_Q4K, 128),
        ("toy-qwen3", mf.QUANT_F32, 128), ("toy-qwen3", mf.QUANT_Q80, 64), ("toy-qwen3", mf.QUANT_Q4K, 128)]
@@ -40,13 +45,9 @@ def test_sort_model_known_answers_oracle(sort_model):
         o.close()
 
 
-@needs_ref
 def test_sort_model_fixture_is_the_embedded_one(sort_model):
-    assert ob.sort_model_bytes() == sort_model
-    r = ob.RefEngine(sort_model, 6, penalty=0.0, temperature=0.0, top_p=0.0, top_k=1)
-    kat = json.load(open(os.path.join(GOLDEN, "sort6_kat.json")))
-    for src, want in kat.items():
-        assert r.seq2seq(src, 6) == want
+    """the committed fixture is byte for byte the model embedded in the reference (its seq2seq answers are sort6_kat.json)"""
+    assert sha(sort_model) == REF_OUT["sort6_model"]
 
 
 @pytest.mark.parametrize("name,quant,gs", TOY)
@@ -65,52 +66,38 @@ def test_oracle_matches_golden_logits(name, quant, gs):
     o.close()
 
 
-@needs_ref
-@pytest.mark.parametrize("name,quant,gs", TOY + [("toy-nano-odd", mf.QUANT_F32, 128), ("mini-qwen3", mf.QUANT_Q80, 128)])
+@pytest.mark.parametrize("name,quant,gs", STRICT_CASES)
 def test_oracle_bit_identical_to_strict_reference(name, quant, gs):
     spec = mf.PRESETS[name]
     path = mf.cached_model(spec, quant, gs)
-    S = 20
-    r = ob.RefEngine(path, S, "strict"); o = ob.NanoOracle(path, S)
-    toks = mf.teacher_tokens(S, spec.vocab)
-    for pos in range(S):
-        assert_bits_equal(r.forward(toks[pos], pos), o.forward(toks[pos], pos), f"{name} pos {pos}")
-    rk, rv = r.kv(); ok, ov = o.kv()
-    assert_bits_equal(rk, ok, "k cache"); assert_bits_equal(rv, ov, "v cache")
-    r.close(); o.close()
+    want = REF_OUT["strict"][f"{name}_{quant:02x}_{gs}"]
+    o = ob.NanoOracle(path, STRICT_SEQ)
+    toks = mf.teacher_tokens(STRICT_SEQ, spec.vocab)
+    for pos in range(STRICT_SEQ):
+        assert sha(o.forward(toks[pos], pos)) == want["logits"][pos], f"{name} pos {pos}: logits differ from the strict reference"
+    ok, ov = o.kv()
+    assert sha(ok) == want["k_cache"], "k cache"
+    assert sha(ov) == want["v_cache"], "v cache"
+    o.close()
 
 
-@needs_ref
 def test_oracle_greedy_with_penalty_matches_reference():
     spec = mf.PRESETS["toy-nano"]
     path = mf.cached_model(spec, mf.QUANT_Q80, 64)
     S, P = 24, 5
-    r = ob.RefEngine(path, S, "strict", penalty=1.3); o = ob.NanoOracle(path, S)
-    ids_r = np.zeros(S + 1, np.uint32); ids_r[:P] = [9, 8, 7, 9, 8]
-    ids_o = ids_r.copy()
+    o = ob.NanoOracle(path, S)
+    ids_o = np.zeros(S + 1, np.uint32); ids_o[:P] = [9, 8, 7, 9, 8]
     for pos in range(S - 1):
-        pre = 1 if pos < P - 1 else 0
-        ids_r[pos + 1] = r.next(ids_r, pos, pre)
-        ids_o[pos + 1] = o.next_greedy(ids_o, pos, pre, 1.3)
-    assert ids_r.tolist() == ids_o.tolist()
-    r.close(); o.close()
+        ids_o[pos + 1] = o.next_greedy(ids_o, pos, 1 if pos < P - 1 else 0, 1.3)
+    assert ids_o.tolist() == REF_OUT["greedy_penalty_1.3_ids"]
+    o.close()
 
 
-@needs_ref
 def test_q4k_writer_matches_reference_quantiser():
     """nano_b200.modelfile.quantize_q4k_blocks (NumPy) == tensor.c:312 quantize_tensor_q4k, byte for byte."""
-    L = ob.RefEngine.lib("strict")
-    rng = np.random.default_rng(7)
-    w = (rng.standard_normal((37, 512), dtype=np.float32) * np.float32(0.05)).astype(np.float32)
-    w[3, :32] = 0.0                       # all-zero group
-    w[5, 32:64] = np.abs(w[5, 32:64])     # all-positive group (bias 0)
-    w[6, 64:96] = -np.abs(w[6, 64:96])    # all-negative group (FLT_TRUE_MIN max quirk)
-    shape = (C.c_uint32 * 2)(37, 512)
-    T = L.quantize_tensor_q4k(w.ctypes.data_as(ob.f32p), 2, shape)
-    nb = L.bytes_num_of_q4k_tensor(T)
-    ref = np.ctypeslib.as_array(C.cast(T, ob.u8p), shape=(nb,)).copy()
+    w = q4k_writer_input()
     mine = mf.q4k_frame((37, 512), 37 * 2) + mf.quantize_q4k_blocks(w).tobytes()
-    assert_bits_equal(np.frombuffer(mine, np.uint8), ref, "q4k tensor bytes")
+    assert sha(mine) == REF_OUT["q4k_tensor"], "q4k tensor bytes"
 
 
 def test_q4k_kat_oracle():
@@ -129,26 +116,18 @@ def test_q4k_kat_oracle():
     assert_bits_equal(mf.quantize_q4k_blocks(W.reshape(8, 768)).reshape(-1), k["w_tensor"][44:], "numpy writer")
 
 
-@needs_ref
 def test_q80_ops_match_reference():
-    L = ob.RefEngine.lib("strict"); O = ob.NanoOracle.lib()
-    rng = np.random.default_rng(3)
-    n, d, gs = 512, 40, 64
-    x = rng.standard_normal(n, dtype=np.float32)
-    x[64:128] = 0.0
-    q_r = np.zeros(n, np.int8); s_r = np.zeros(n // gs, np.float32)
-    t = ob.Q80Tensor(q_r.ctypes.data_as(ob.i8p), s_r.ctypes.data_as(ob.f32p))
-    L.quantize(C.byref(t), x.ctypes.data_as(ob.f32p), n, gs)
+    O = ob.NanoOracle.lib()
+    x, wq, ws, n, d, gs = q80_ops_inputs()
     q_o = np.zeros(n, np.int8); s_o = np.zeros(n // gs, np.float32)
     O.nor_q80_quantize(q_o.ctypes.data_as(ob.i8p), s_o.ctypes.data_as(ob.f32p), x.ctypes.data_as(ob.f32p), n, gs)
-    assert_bits_equal(q_r, q_o, "codes"); assert_bits_equal(s_r, s_o, "scales")
-    wq, ws = mf.quantize_q80(rng.standard_normal((d, n), dtype=np.float32) * 0.02, gs)
-    tw = ob.Q80Tensor(wq.ctypes.data_as(ob.i8p), ws.ctypes.data_as(ob.f32p))
-    y_r = np.zeros(d, np.float32); y_o = np.zeros(d, np.float32)
-    L.matmul_quant(y_r.ctypes.data_as(ob.f32p), C.byref(t), C.byref(tw), n, d, gs)
+    want = REF_OUT["q80_ops"]
+    assert sha(q_o) == want["codes"], "codes"
+    assert sha(s_o) == want["scales"], "scales"
+    y_o = np.zeros(d, np.float32)
     O.nor_matvec_q80(y_o.ctypes.data_as(ob.f32p), q_o.ctypes.data_as(ob.i8p), s_o.ctypes.data_as(ob.f32p),
                      wq.ctypes.data_as(ob.i8p), ws.ctypes.data, n, d, gs)
-    assert_bits_equal(y_r, y_o, "matmul_quant")
+    assert sha(y_o) == want["matmul_quant"], "matmul_quant"
 
 
 def test_expf_ref_equals_host_libm():
@@ -165,24 +144,17 @@ def test_expf_ref_equals_host_libm():
         assert_bits_equal(E.host_expf_ref(x), want, "expf")
 
 
-@needs_ref
 def test_lora_golden_is_what_the_reference_computes():
-    """Pins tests/golden/lora_logits.npz (the GPU LoRA tests' fixture) to the unmodified strict reference with the same
-    synthetic plug-in, and checks that the plug-in writer's layout is the one parse_lora_file reads (infer.c:436-500)."""
+    """Pins tests/golden/lora_logits.npz (the GPU LoRA tests' fixture) to the strict reference's digests with the same synthetic
+    plug-in, checks that the plug-in writer's layout is the one parse_lora_file reads (infer.c:436-500), and that the plug-in
+    changes the reference's logits (toy_logits.npz holds them without it)."""
     spec = mf.PRESETS["toy-nano"]
     lora = mf.write_lora(spec, 8, 16, seed=7)
     assert len(lora) == 256 + 4 * spec.n_layer * 8 * (4 * spec.n_embd + 2 * spec.n_embd + 2 * spec.kv_dim)
     gold = np.load(os.path.join(GOLDEN, "lora_logits.npz"))
-    for quant, gs in [(mf.QUANT_F32, 128), (mf.QUANT_Q80, 64)]:
-        path = mf.cached_model(spec, quant, gs)
-        plain = ob.RefEngine(path, 24, "strict")
-        r = ob.RefEngine(path, 24, "strict"); r.load_lora(lora)
-        toks = mf.teacher_tokens(24, spec.vocab)
-        rows = []
-        for pos in range(24):
-            lg = r.forward(toks[pos], pos); base = plain.forward(toks[pos], pos)
-            if pos in (0, 1, 7, 23):
-                rows.append(lg)
-                assert np.abs(lg - base).max() > 1e-2, "the plug-in must change the logits"
-        assert_bits_equal(np.stack(rows), gold[f"toy-nano_{quant:02x}_{gs}"], f"lora golden {quant:#x}")
-        r.close(); plain.close()
+    base = np.load(os.path.join(GOLDEN, "toy_logits.npz"))
+    for quant, gs in LORA_CASES[:2]:
+        key = f"toy-nano_{quant:02x}_{gs}"
+        for i, pos in enumerate(TOY_POSITIONS):
+            assert sha(gold[key][i]) == REF_OUT["lora"][key]["logits"][pos], f"lora golden {quant:#x} pos {pos}"
+            assert np.abs(gold[key][i] - base[key][i]).max() > 1e-2, "the plug-in must change the logits"

@@ -13,7 +13,7 @@ from nano_b200 import build as nb_build
 from oracle import bindings as ob
 
 REF_SO = os.path.join(ob.REF_DIR, "libnano_ref_strict.so")
-pytestmark = pytest.mark.skipif(not (os.path.exists(REF_SO) and os.path.exists(nb_build.SHIM_SO) and os.path.exists(nb_build.REFHOST_SO)),
+pytestmark = pytest.mark.skipif(not (os.path.exists(REF_SO) and os.path.exists(nb_build.SHIM_SO) and os.path.exists(ob.REFHOST_SO)),
                                 reason="needs oracle/_ref (reference build) and the shim libraries")
 
 f32p, u32p, u8p = C.POINTER(C.c_float), C.POINTER(C.c_uint32), C.POINTER(C.c_uint8)
@@ -41,7 +41,7 @@ def _proto(L):
 
 @pytest.fixture(scope="module")
 def libs():
-    C.CDLL(nb_build.REFHOST_SO, mode=C.RTLD_GLOBAL)            # the reference's tokenizer / utils / HAL objects the shim links against
+    C.CDLL(ob.REFHOST_SO, mode=C.RTLD_GLOBAL)            # the reference's tokenizer / utils / HAL objects the shim links against
     ref = _proto(C.CDLL(REF_SO, mode=C.RTLD_LOCAL))
     ref.quantize_tensor_q4k.restype = C.c_void_p
     ref.quantize_tensor_q4k.argtypes = [f32p, C.c_uint32, u32p]

@@ -1,4 +1,4 @@
-// Microbenchmark: cost of grid-barrier variants on B200 (148 CTAs x 512 threads, cooperative launch).
+// Microbenchmark: cost of grid-barrier variants (one CTA per SM x 512 threads, cooperative launch; flags sized for up to 148 SMs).
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <stdint.h>

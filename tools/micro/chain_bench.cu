@@ -177,7 +177,8 @@ int main() {
     CK(cudaMemcpy(x, h, sizeof h, cudaMemcpyHostToDevice));
     unsigned long long hw[4096]; for (int i = 0; i < 4096; i++) hw[i] = (7ull << 32) | (unsigned)i;
     CK(cudaMemcpy(words, hw, sizeof hw, cudaMemcpyHostToDevice));
-    for (int ncta : {1, 148}) {
+    int sms = 0; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+    for (int ncta : {1, sms}) {
         k_chain<<<ncta, 512>>>(x, words, out, 200);
         CK(cudaDeviceSynchronize());
         long long r[12]; CK(cudaMemcpy(r, out, 96, cudaMemcpyDeviceToHost));

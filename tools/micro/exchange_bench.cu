@@ -1,4 +1,4 @@
-// Microbenchmark: the bare activation-exchange protocol of k_decode_stream.  148 CTAs x 480 threads; per round every CTA publishes
+// Microbenchmark: the bare activation-exchange protocol of k_decode_stream.  One CTA per SM x 480 threads; per round every CTA publishes
 // its share of an n-element vector as {value, epoch} words into R replicas (st.relaxed.gpu), then all its threads poll the words
 // of their slot in "their" replica until the round's epoch has arrived (ld.relaxed.gpu.v2.u64 x 2), bar.sync, next round.
 // Reports cycles per round = the floor of a decode phase with no arithmetic at all.
@@ -43,7 +43,7 @@ int main() {
     unsigned long long *buf; long long *out;
     CK(cudaMalloc(&buf, 8 * 4096 * 8)); CK(cudaMalloc(&out, 64));
     for (uint32_t n : {768u, 1920u})
-        for (uint32_t R : {1u, 8u})
+        for (uint32_t R : {1u, 4u, 8u})
             for (int sl : {0, 50})
                 for (int pollers : {480, 64}) {
                     CK(cudaMemset(buf, 0, 8 * 4096 * 8));

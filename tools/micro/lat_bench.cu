@@ -1,5 +1,5 @@
-// Microbenchmark: the latencies the persistent decode kernel is made of, measured on an otherwise idle B200 and with
-// the other 147 SMs polling L2 (the situation inside a grid barrier).
+// Microbenchmark: the latencies the persistent decode kernel is made of, measured on an otherwise idle GPU and with
+// all other SMs polling L2 (the situation inside a grid barrier).
 //   * dependent ld.global.cg / ld.relaxed.gpu / ld.acquire.gpu chain through an L2-resident buffer (cycles per load)
 //   * st.global + fence (membar.gl) drain time, atomicAdd round trip
 //   * cp.async.bulk of 8 KB: issue -> mbarrier completion, source in L2 and in HBM
