@@ -53,7 +53,10 @@ __device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src_gmem, u
                  ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 // A spin that cannot hang the GPU: after ~2 s the kernel records a code and traps (the host sees a launch failure).
-static __device__ __noinline__ void st_give_up(uint32_t *err, uint32_t code) {
+// The spins themselves are inline.  A call to an out-of-line function makes its caller save every live register to the
+// stack (local memory) around the call, and with the consumers' state at the 128-register cap that put spill stores and
+// reloads on the hot path of every phase.  The give-up is out of line but never returns, so its call sites save nothing.
+[[noreturn]] static __device__ __noinline__ void st_give_up(uint32_t *err, uint32_t code) {
     if (err) *err = code;
     __threadfence_system();
     __trap();
@@ -61,16 +64,17 @@ static __device__ __noinline__ void st_give_up(uint32_t *err, uint32_t code) {
 // A polling warp must not monopolise the SM's MIO pipe (mbarrier, shared-memory and shuffle instructions share it): measured with
 // the producer busy-polling a full ring, a 5-step warp shuffle reduction in a consumer warp took ~1000 cycles instead of ~150.
 // `sleep_ns` > 0: back off between polls (the producer runs ahead of the consumers and is never latency-critical).
-static __device__ __noinline__ void mbar_wait_slow(uint64_t *bar, uint32_t parity, uint32_t *err, uint32_t code, uint32_t sleep_ns) {
+__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity, uint32_t *err, uint32_t code, uint32_t sleep_ns = 20) {
+    if (mbar_try_wait(bar, parity)) return;
     const long long t0 = clock64();
     while (!mbar_try_wait(bar, parity)) {
         if (sleep_ns) __nanosleep(sleep_ns);
         if (clock64() - t0 > 4000000000ll) st_give_up(err, code);
     }
 }
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity, uint32_t *err, uint32_t code, uint32_t sleep_ns = 20) {
-    if (!mbar_try_wait(bar, parity)) mbar_wait_slow(bar, parity, err, code, sleep_ns);
-}
+// threadIdx.x through an opaque read, in the consumers' device functions: the compiler cannot hoist what is derived from it
+// (lane offsets, slot indices) out of the layer loop, where it would stay live across every phase (128-register cap)
+__device__ __forceinline__ uint32_t st_tid() { uint32_t t; asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t)); return t; }
 // barrier among the 15 consumer warps only (the producer warp never takes part)
 __device__ __forceinline__ void cbar() { asm volatile("bar.sync 1, %0;" ::"n"(kConsThreads) : "memory"); }
 
@@ -90,26 +94,24 @@ constexpr uint32_t kXwAny = 0xffffffffu;        // timing experiments only (NB20
 __device__ __forceinline__ bool xw_ok(unsigned long long w, uint32_t need) { return (uint32_t)(w >> 32) == need || need == kXwAny; }
 __device__ __forceinline__ float xw_val(unsigned long long w) { return __uint_as_float((uint32_t)w); }
 // 4 consecutive words (32-byte aligned) -> float4 once all of them carry `need`
-static __device__ __noinline__ float4 xw_poll4_slow(const unsigned long long *p, uint32_t need, uint32_t *err) {
+// a failed poll of a spin: the clock is read every 256th time only (the loop stays loads and compares), give up after ~2 s
+__device__ __forceinline__ void xw_spin_guard(uint32_t it, long long &t0, uint32_t *err, uint32_t code) {
+    if ((it & 255u) == 0) {
+        if (t0 == 0) t0 = clock64();
+        else if (clock64() - t0 > 4000000000ll) st_give_up(err, code);
+    }
+}
+__device__ __forceinline__ float4 xw_poll4(const unsigned long long *p, uint32_t need, uint32_t *err) {
     unsigned long long a, b, c, d;
     long long t0 = 0;
     for (uint32_t it = 1;; it++) {
         xw_ld2(p, a, b); xw_ld2(p + 2, c, d);
         if (xw_ok(a, need) && xw_ok(b, need) && xw_ok(c, need) && xw_ok(d, need)) break;
-        if ((it & 255u) == 0) {                      // the clock is read rarely: the loop stays a pair of loads and four compares
-            if (t0 == 0) t0 = clock64();
-            else if (clock64() - t0 > 4000000000ll) st_give_up(err, 0x50u);
-        }
+        xw_spin_guard(it, t0, err, 0x50u);
     }
     return make_float4(xw_val(a), xw_val(b), xw_val(c), xw_val(d));
 }
-__device__ __forceinline__ float4 xw_poll4(const unsigned long long *p, uint32_t need, uint32_t *err) {
-    unsigned long long a, b, c, d;
-    xw_ld2(p, a, b); xw_ld2(p + 2, c, d);
-    if (xw_ok(a, need) && xw_ok(b, need) && xw_ok(c, need) && xw_ok(d, need)) return make_float4(xw_val(a), xw_val(b), xw_val(c), xw_val(d));
-    return xw_poll4_slow(p, need, err);
-}
-static __device__ __noinline__ float xw_poll1(const unsigned long long *p, uint32_t need, uint32_t *err) {
+__device__ __forceinline__ float xw_poll1(const unsigned long long *p, uint32_t need, uint32_t *err) {
     unsigned long long a = xw_ld1(p);
     if (!xw_ok(a, need)) {
         const long long t0 = clock64();
@@ -151,6 +153,8 @@ __device__ __forceinline__ void mbar_arrive_n(uint64_t *bar, uint32_t n) {
 struct StCursor { uint32_t s, par; };     // stage and parity of the next tile (producer: empty parity; consumer: full parity)
 __device__ __forceinline__ void st_advance(StCursor &c, uint32_t nstages) { if (++c.s == nstages) { c.s = 0; c.par ^= 1u; } }
 struct StOwn { uint32_t row0[5], rows[5]; };      // the rows this CTA owns of every phase kind (shared memory; computed once)
+// the consumers' token state (shared memory, identical in every CTA; thread 0 advances it at the end of a token)
+struct StStep { uint32_t step, pos, tok, range, nsplit, chunk, causal, n_prompt, advance; float pen; };
 // How the 32 lanes of a warp share the rows of a tile, per phase kind (computed once per launch, kept in shared memory:
 // run-time integer divisions cost ~150 cycles each and sat on every phase's critical path).
 // Q80: a row of G groups is owned by a team of gteam * lg2 lanes (lg2 lanes split the 16-byte chunks of one group);
@@ -238,13 +242,15 @@ static __device__ void st_producer(const StreamArgs &g, const StRing &r, const S
 #else
 #define ST_DBG(k) do { } while (0)
 #endif
+constexpr int kStPollB = 2;          // Q80 / F32 warp slots whose exchange words are polled together
+static_assert(kStKmax % kStPollB == 0, "stream kernel: poll batches cover the warp slots");
 template <int QUANT, int LPG>
 __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long long *xsrc, const float *ssrc, uint32_t need, const float *__restrict__ gain,
                                         uint32_t n, unsigned char *act, float *red, unsigned long long *dbg) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int lane = st_tid() & 31, warp = st_tid() >> 5;
     ST_DBG(0);
     if (gain) {      // the gain is applied after the sum of squares: start pulling its lines into L1 while the source is awaited
-        for (uint32_t i = threadIdx.x * 32u; i < n; i += kConsThreads * 32u) asm volatile("prefetch.global.L1 [%0];" ::"l"(gain + i));
+        for (uint32_t i = st_tid() * 32u; i < n; i += kConsThreads * 32u) asm volatile("prefetch.global.L1 [%0];" ::"l"(gain + i));
     }
     auto nrm = [&](float4 v, float4 gn, float inv) -> float4 {      // infer.c:611: weight * (ss * x)
         return make_float4(__fmul_rn(gn.x, __fmul_rn(inv, v.x)), __fmul_rn(gn.y, __fmul_rn(inv, v.y)),
@@ -312,35 +318,63 @@ __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long
         static_assert(LG == 16 || LG == 32, "stream kernel: Q80 group size 64 or 128");
         const uint32_t G = (n + gs - 1u) / gs;                           // F32: n % 4 == 0 only, the last slot may be partial
         const uint32_t sub = lane / LG, li = lane % LG;
-        float4 v[kStKmax];
-        if (ssrc) {
-#pragma unroll
-            for (int j = 0; j < kStKmax; j++) {
-                const uint32_t i = ((warp + kConsWarps * j) * GW + sub) * gs + li * 4u;
-                v[j] = (i < n) ? *reinterpret_cast<const float4 *>(ssrc + i) : make_float4(0, 0, 0, 0);
-            }
-        } else {
-            // every load of the thread is in flight before the first epoch is looked at
-            unsigned long long w[kStKmax][4];
-#pragma unroll
-            for (int j = 0; j < kStKmax; j++) {
-                const uint32_t i = ((warp + kConsWarps * j) * GW + sub) * gs + li * 4u;
-                if (i < n) { xw_ld2(xsrc + i, w[j][0], w[j][1]); xw_ld2(xsrc + i + 2, w[j][2], w[j][3]); }
-            }
-#pragma unroll
-            for (int j = 0; j < kStKmax; j++) {
-                const uint32_t i = ((warp + kConsWarps * j) * GW + sub) * gs + li * 4u;
-                v[j] = make_float4(0, 0, 0, 0);
-                if (i < n) {
-                    if (xw_ok(w[j][0], need) && xw_ok(w[j][1], need) && xw_ok(w[j][2], need) && xw_ok(w[j][3], need))
-                        v[j] = make_float4(xw_val(w[j][0]), xw_val(w[j][1]), xw_val(w[j][2]), xw_val(w[j][3]));
-                    else v[j] = xw_poll4_slow(xsrc + i, need, g.err);
+        auto slot_i = [&](int j) -> uint32_t { return ((warp + kConsWarps * j) * GW + sub) * gs + li * 4u; };
+        // a slot's 4 values (0 past n) once they are known to have arrived: shared source, or exchange words already polled
+        auto reread = [&](int j) -> float4 {
+            const uint32_t i = slot_i(j);
+            float4 a = make_float4(0, 0, 0, 0);
+            if (i < n) {
+                if (ssrc) a = *reinterpret_cast<const float4 *>(ssrc + i);
+                else {
+                    unsigned long long w0, w1, w2, w3;
+                    xw_ld2(xsrc + i, w0, w1); xw_ld2(xsrc + i + 2, w2, w3);
+                    a = make_float4(xw_val(w0), xw_val(w1), xw_val(w2), xw_val(w3));
                 }
             }
-        }
+            return a;
+        };
+        // The slots are read in batches of kStPollB: every load of a batch is in flight before its first epoch is looked at,
+        // and a batch that is not complete is polled again whole.  Every n <= 15 * kStPollB * 128 (all phases of Nano and
+        // Qwen3-0.6B) is one batch, i.e. one round trip.  Only the first batch stays in registers until the quantise pass;
+        // later batches are read again there (their words cannot change before this CTA has published its next exchange).
+        // Holding all six slots took 48 staging + 24 value registers and spilled to local memory on every phase.
+        float4 v[kStPollB];
         float ss = 0.0f;
 #pragma unroll
-        for (int j = 0; j < kStKmax; j++) ss = sq(v[j], ss);
+        for (int j0 = 0; j0 < kStKmax; j0 += kStPollB) {
+            float4 vb[kStPollB];
+            if (ssrc) {
+#pragma unroll
+                for (int b = 0; b < kStPollB; b++) vb[b] = reread(j0 + b);
+            } else {
+                unsigned long long w[kStPollB][4];
+                long long t0 = 0;
+                for (uint32_t it = 1;; it++) {
+                    bool ok = true;
+#pragma unroll
+                    for (int b = 0; b < kStPollB; b++) {
+                        // defined on every path (a slot past n reads as 0.0f): a register written only under a predicate
+                        // stays live around the layer loop, as the compiler cannot see that it is never read unwritten
+                        w[b][0] = w[b][1] = w[b][2] = w[b][3] = 0ull;
+                        const uint32_t i = slot_i(j0 + b);
+                        if (i < n) { xw_ld2(xsrc + i, w[b][0], w[b][1]); xw_ld2(xsrc + i + 2, w[b][2], w[b][3]); }
+                    }
+#pragma unroll
+                    for (int b = 0; b < kStPollB; b++) {
+                        if (slot_i(j0 + b) < n) ok = ok && xw_ok(w[b][0], need) && xw_ok(w[b][1], need) && xw_ok(w[b][2], need) && xw_ok(w[b][3], need);
+                    }
+                    if (ok) break;
+                    xw_spin_guard(it, t0, g.err, 0x50u);
+                }
+#pragma unroll
+                for (int b = 0; b < kStPollB; b++) vb[b] = make_float4(xw_val(w[b][0]), xw_val(w[b][1]), xw_val(w[b][2]), xw_val(w[b][3]));
+            }
+#pragma unroll
+            for (int b = 0; b < kStPollB; b++) {
+                ss = sq(vb[b], ss);                                   // slot order, as one pass over all slots
+                if (j0 == 0) v[b] = vb[b];
+            }
+        }
         ST_DBG(1);
         float inv = 1.0f;
         if (gain && !(g.ablate & 8u)) inv = inverse(ss);
@@ -351,7 +385,7 @@ __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long
             if (g0 < G) {                                            // warp-uniform
                 const uint32_t gi = g0 + sub, i = gi * gs + li * 4u;
                 const bool on = i < n;
-                float4 a = v[j];
+                float4 a = (j < kStPollB) ? v[j] : reread(j);
                 if (gain && on) a = nrm(a, __ldg(reinterpret_cast<const float4 *>(gain + i)), inv);
                 if constexpr (QUANT == 0x00) {
                     if (on) *reinterpret_cast<float4 *>(act + (size_t)i * 4u) = a;
@@ -380,11 +414,15 @@ __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long
                                 tie = tie || fabsf(aq - cf) > 0.499f;
                                 cq[u] = q < 0.0f ? -c : c;
                             }
-                            if (tie) {                                           // rare: some q within 1e-3 of a tie -> the exact division + round()
-#pragma unroll
-                                for (int u = 0; u < 4; u++) cq[u] = q80_code_slow(av[u], sc);
-                            }
                             pk = ((uint32_t)cq[0] & 0xffu) | (((uint32_t)cq[1] & 0xffu) << 8) | (((uint32_t)cq[2] & 0xffu) << 16) | (((uint32_t)cq[3] & 0xffu) << 24);
+                            if (tie) {                                           // rare: some q within 1e-3 of a tie -> the exact division + round()
+                                pk = 0;                                          // (inline, one division site per slot: q80_code_slow is a call)
+#pragma unroll 1
+                                for (uint32_t u = 0; u < 4u; u++) {
+                                    const float x = u == 0u ? a.x : u == 1u ? a.y : u == 2u ? a.z : a.w;
+                                    pk |= ((uint32_t)(int)roundf(__fdiv_rn(x, sc)) & 0xffu) << (8u * u);
+                                }
+                            }
                         }
                         *reinterpret_cast<uint32_t *>(codes + i) = pk;
                         if (li == 0) scales[gi] = sc;
@@ -448,7 +486,7 @@ template <int LPG, int RB>
 __device__ __forceinline__ void st_rows_q80_warp(const unsigned char *wrow, uint32_t row_stride, const unsigned char *srow, uint32_t aux_stride,
                                                  uint32_t n, const unsigned char *act, float (&val)[RB]) {
     constexpr uint32_t gs = LPG * 16;
-    const int lane = threadIdx.x & 31;
+    const int lane = st_tid() & 31;
     const float *xs = reinterpret_cast<const float *>(act + ((n + 15u) & ~15u));
     float acc[RB];
 #pragma unroll
@@ -475,7 +513,7 @@ __device__ __forceinline__ void st_rows_q80_warp(const unsigned char *wrow, uint
 }
 // F32: matmul infer.c:637-651, fast mode (one warp per row: lane-split FMA + tree)
 __device__ __forceinline__ float st_row_f32(const unsigned char *wrow, uint32_t n, const unsigned char *act) {
-    const int lane = threadIdx.x & 31;
+    const int lane = st_tid() & 31;
     const float *x = reinterpret_cast<const float *>(act);
     float acc = 0.0f;
 #pragma unroll 2
@@ -487,7 +525,7 @@ __device__ __forceinline__ float st_row_f32(const unsigned char *wrow, uint32_t 
 }
 // Q4K: matmul_q4k / dot_two_blocks_q4k tensor.c:359-471 (one warp per row; one lane = one 32-element group per step; side: 20-byte records)
 __device__ __forceinline__ float st_row_q4k(const unsigned char *wrow, const unsigned char *side, uint32_t n, const unsigned char *act) {
-    const int lane = threadIdx.x & 31;
+    const int lane = st_tid() & 31;
     const uint32_t *xe = reinterpret_cast<const uint32_t *>(act);
     const uint32_t *xo = reinterpret_cast<const uint32_t *>(act + n / 2);
     const float4 *gp = reinterpret_cast<const float4 *>(act + n);
@@ -538,7 +576,7 @@ __device__ __forceinline__ void st_consume(const StreamArgs &g, const StRing &r,
                                            uint32_t row0, uint32_t rows, uint32_t epoch, const unsigned char *act, uint32_t pos, float pen,
                                            float *xown, MatvecSmem &ms, const StGeo &geo, uint32_t kid, unsigned long long *dbg) {
     const Dims &d = g.d;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int lane = st_tid() & 31, warp = st_tid() >> 5;
     float bestv = -FLT_MAX; uint32_t besti = 0xffffffffu;
     // epilogue of one finished row (value in all `ts` lanes of its team; `ri` = index among the rows this CTA owns)
     auto emit = [&](uint32_t row, uint32_t ri, float v, float v3, bool pub, uint32_t tl, uint32_t ts) {
@@ -585,9 +623,16 @@ __device__ __forceinline__ void st_consume(const StreamArgs &g, const StRing &r,
                 const unsigned char *tile = r.buf + (size_t)cc.s * r.stage_bytes;
                 const unsigned char *aux = tile + (size_t)tr * k.row_stride;
                 // rows in blocks of 4 / 2 / 1 (SwiGLU tiles hold whole (w1, w3) pairs: an even row count)
-                auto out = [&](uint32_t rr, const float *v, uint32_t cnt) {
-                    if (epi == EPI_SWIGLU) { for (uint32_t u = 0; u + 1u < cnt; u += 2u) emit(row0 + done + rr + u, done + rr + u, v[u], v[u + 1u], true, (uint32_t)lane, 32u); }
-                    else { for (uint32_t u = 0; u < cnt; u++) emit(row0 + done + rr + u, done + rr + u, v[u], 0.0f, true, (uint32_t)lane, 32u); }
+                // (unrolled over the block size: a run-time index into v would put it in local memory)
+                auto out = [&](uint32_t rr, const auto &v, uint32_t cnt) {
+                    constexpr uint32_t RB = sizeof(v) / sizeof(v[0]);
+                    if (epi == EPI_SWIGLU) {
+#pragma unroll
+                        for (uint32_t u = 0; u + 1u < RB; u += 2u) if (u + 1u < cnt) emit(row0 + done + rr + u, done + rr + u, v[u], v[u + 1u], true, (uint32_t)lane, 32u);
+                    } else {
+#pragma unroll
+                        for (uint32_t u = 0; u < RB; u++) if (u < cnt) emit(row0 + done + rr + u, done + rr + u, v[u], 0.0f, true, (uint32_t)lane, 32u);
+                    }
                 };
                 uint32_t rr = 0;
                 if constexpr (QUANT == 0x80) {
@@ -701,7 +746,7 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
     const float *qn = g.qnorm ? g.qnorm + (size_t)layer * hd : nullptr, *kn = g.knorm ? g.knorm + (size_t)layer * hd : nullptr;
     const float *cr = g.rope_cos + (size_t)pos * (hd / 2), *ci = g.rope_sin + (size_t)pos * (hd / 2);
     uint32_t lpr = 1; while (lpr * 4 < hd) lpr <<= 1;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int lane = st_tid() & 31, warp = st_tid() >> 5;
     const uint32_t li = lane % lpr, col = li * 4;
     const bool colon = col < hd;
     const float dv = sqrtf((float)hd);
@@ -747,23 +792,19 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
 
     for (uint32_t s0 = t0; s0 < t1; s0 += seg_max) {
         const uint32_t rows_seg = min(seg_max, t1 - s0), nt = (rows_seg + kvr - 1u) / kvr;
-        uint32_t stg[kStSegTiles];
+        unsigned long long stg = 0;                    // ring stage of resident tile i in byte i (two registers, not kStSegTiles)
+        static_assert(kStSegTiles <= 8 && kStMaxStages <= 256, "stream kernel: stage indices packed in bytes");
 #pragma unroll
         for (int i = 0; i < kStSegTiles; i++) {
-            stg[i] = 0;
-            if ((uint32_t)i < nt) { mbar_wait(&r.full[c.s], c.par, g.err, 0x30u); stg[i] = c.s; st_advance(c, r.nstages); tcount++; }
+            if ((uint32_t)i < nt) { mbar_wait(&r.full[c.s], c.par, g.err, 0x30u); stg |= (unsigned long long)c.s << (8 * i); st_advance(c, r.nstages); tcount++; }
         }
-        auto tile_k = [&](uint32_t ti) -> float * {
-            uint32_t sidx = stg[0];
-#pragma unroll
-            for (int i = 1; i < kStSegTiles; i++) if (ti == (uint32_t)i) sidx = stg[i];
-            return reinterpret_cast<float *>(r.buf + (size_t)sidx * r.stage_bytes);
-        };
+        auto stage_of = [&](uint32_t ti) -> uint32_t { return (uint32_t)(stg >> (8u * ti)) & 0xffu; };
+        auto tile_k = [&](uint32_t ti) -> float * { return reinterpret_cast<float *>(r.buf + (size_t)stage_of(ti) * r.stage_bytes); };
         ST_DBG(2);
         if (owns && pos >= s0 && pos < s0 + rows_seg) {     // CTA-uniform: this step's k / v into their slots of the resident tile
             const uint32_t pr = pos - s0, ti = __umulhi(pr, g.kv_tile_magic), rr = pr - ti * kvr;
             float *kt = tile_k(ti);
-            for (uint32_t i = threadIdx.x; i < hd; i += kConsThreads) {
+            for (uint32_t i = st_tid(); i < hd; i += kConsThreads) {
                 kt[(size_t)rr * hd + i] = krow[i];
                 kt[(size_t)kvr * hd + (size_t)rr * hd + i] = krow[hd + i];
             }
@@ -774,8 +815,8 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
         //      all KVM query heads (q chunks are broadcast reads); chunk order rotated by the row index: conflict-free although rows are
         //      a multiple of 128 bytes apart.  One round covers 120 rows. ----
         if (!(g.ablate & 4u)) {
-            const uint32_t part = threadIdx.x & 3u;
-            for (uint32_t idx = threadIdx.x >> 2; idx < ((rows_seg + 7u) & ~7u); idx += kConsThreads / 4u) {       // warp-uniform trip count (8 rows per warp)
+            const uint32_t part = st_tid() & 3u;
+            for (uint32_t idx = st_tid() >> 2; idx < ((rows_seg + 7u) & ~7u); idx += kConsThreads / 4u) {       // warp-uniform trip count (8 rows per warp)
                 const bool on = idx < rows_seg;
                 const uint32_t ic = on ? idx : 0u;
                 const uint32_t ti = __umulhi(ic, g.kv_tile_magic), rr = ic - ti * kvr;
@@ -784,7 +825,8 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
                 float a[KVM];
 #pragma unroll
                 for (int m = 0; m < KVM; m++) a[m] = 0.0f;
-#pragma unroll 4
+                constexpr int kUnroll = KVM >= 4 ? 2 : 4;      // KVM = 4: 4 chunks in flight held ~80 registers and spilled
+#pragma unroll kUnroll
                 for (uint32_t cc = part; cc < hd4; cc += 4u) {
                     uint32_t ch = cc + rot; if (ch >= hd4) ch -= hd4;
                     const float4 k4 = *reinterpret_cast<const float4 *>(kr + ch * 4u);
@@ -828,7 +870,7 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
         // ---- P.V: thread j owns (head, dim pair) j; rows in order, four at a time (probabilities as one float4) ----
 #pragma unroll
         for (int u = 0; u < 2; u++) {
-            const uint32_t j = threadIdx.x + u * kConsThreads;
+            const uint32_t j = st_tid() + u * kConsThreads;
             if (j < KVM * hd2 && !(g.ablate & 4u)) {
                 const uint32_t m = j / hd2, dd = (j - m * hd2) * 2u;
                 const float *Sm = S + m * seg_max;
@@ -858,14 +900,14 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
         ST_DBG(6);
         if (lane == 0) {
 #pragma unroll
-            for (int i = 0; i < kStSegTiles; i++) if ((uint32_t)i < nt) mbar_arrive(&r.empty[stg[i]]);
+            for (int i = 0; i < kStSegTiles; i++) if ((uint32_t)i < nt) mbar_arrive(&r.empty[stage_of(i)]);
         }
     }
     ST_DBG(7);
     // ---- the item's partial: per head [acc[hd], M, L] ----
 #pragma unroll
     for (int u = 0; u < 2; u++) {
-        const uint32_t j = threadIdx.x + u * kConsThreads;
+        const uint32_t j = st_tid() + u * kConsThreads;
         if (j < KVM * hd2) { const uint32_t m = j / hd2, dd = (j - m * hd2) * 2u; outp[m * (hd + 2) + dd] = acc[u].x; outp[m * (hd + 2) + dd + 1u] = acc[u].y; }
     }
     if (warp < KVM && lane == 0) { outp[warp * (hd + 2) + hd] = m_run; outp[warp * (hd + 2) + hd + 1] = l_run; }
@@ -873,7 +915,7 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
     cbar();
     ST_DBG(8);
     if (nsplit == 1) {          // the whole range in one item: normalise and publish
-        for (uint32_t el = threadIdx.x; el < KVM * hd; el += kConsThreads) {
+        for (uint32_t el = st_tid(); el < KVM * hd; el += kConsThreads) {
             const uint32_t m = el / hd, i = el - m * hd;
             const float ov = __fdiv_rn(outp[m * (hd + 2) + i], outp[m * (hd + 2) + hd + 1]);
 #pragma unroll
@@ -883,7 +925,7 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
     }
     unsigned long long *part = g.xws + ((size_t)kvh * g.nsplit_max) * pw;
     if (sp != 0) {              // publish the partial; split 0 of the kv head merges
-        for (uint32_t idx = threadIdx.x; idx < pw; idx += kConsThreads) xw_st(part + (size_t)sp * pw + idx, outp[idx], e_out);
+        for (uint32_t idx = st_tid(); idx < pw; idx += kConsThreads) xw_st(part + (size_t)sp * pw + idx, outp[idx], e_out);
         return;
     }
     ST_DBG(9);
@@ -894,7 +936,7 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
     float *stat = wsc + KVM * g.nsplit_max;              // [KVM] L, then [KVM][nsplit_max] partial sums
     float own[4];                                        // this thread's slice of the own partial (pw <= 4 * 480 for hd <= 128, KVM <= 8)
 #pragma unroll
-    for (int u = 0; u < 4; u++) { const uint32_t idx = threadIdx.x + u * kConsThreads; own[u] = idx < pw ? outp[idx] : 0.0f; }
+    for (int u = 0; u < 4; u++) { const uint32_t idx = st_tid() + u * kConsThreads; own[u] = idx < pw ? outp[idx] : 0.0f; }
     cbar();                                              // outp / ws are about to be overwritten by the staging area
     float *macc = sm;                                    // [KVM][nsplit][hd]
     float *pl = stat + KVM;                              // [KVM][nsplit_max]
@@ -905,8 +947,8 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
         else pl[m * g.nsplit_max + s2] = v;
     };
 #pragma unroll
-    for (int u = 0; u < 4; u++) { const uint32_t idx = threadIdx.x + u * kConsThreads; if (idx < pw) place(0, idx, own[u]); }
-    for (uint32_t e0 = pw + threadIdx.x; e0 < nsplit * pw; e0 += 8u * kConsThreads) {       // eight loads in flight per thread before any epoch is checked
+    for (int u = 0; u < 4; u++) { const uint32_t idx = st_tid() + u * kConsThreads; if (idx < pw) place(0, idx, own[u]); }
+    for (uint32_t e0 = pw + st_tid(); e0 < nsplit * pw; e0 += 8u * kConsThreads) {       // eight loads in flight per thread before any epoch is checked
         unsigned long long w8[8];
 #pragma unroll
         for (int u = 0; u < 8; u++) { const uint32_t e = e0 + u * kConsThreads; if (e < nsplit * pw) w8[u] = xw_ld1(part + e); }
@@ -938,7 +980,7 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
         if (lane == 0) stat[warp] = L;
     }
     cbar();
-    for (uint32_t el = threadIdx.x; el < KVM * hd; el += kConsThreads) {
+    for (uint32_t el = st_tid(); el < KVM * hd; el += kConsThreads) {
         const uint32_t m = el / hd, i = el - m * hd;
         float o = 0.0f;
         for (uint32_t s2 = 0; s2 < nsplit; s2++) o = fmaf(macc[(m * nsplit + s2) * hd + i], wsc[m * g.nsplit_max + s2], o);
@@ -952,7 +994,7 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
 // ---------------------------------------------------------------- grid barrier, once per token (consumer warps; the producer keeps streaming)
 __device__ __forceinline__ void st_grid_barrier(const StreamArgs &g, unsigned int &target_smem, volatile uint32_t *progress, uint32_t ncta) {
     cbar();
-    if (threadIdx.x == 0) {
+    if (st_tid() == 0) {
         const unsigned int target = target_smem + ncta;
         target_smem = target;
         asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(g.bar) : "memory");       // release: this CTA's plain stores of the token
@@ -984,14 +1026,22 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
     __shared__ float xown[kStOwnMax];
     __shared__ volatile uint32_t s_progress;
     __shared__ unsigned int s_target;
+    __shared__ StStep ss;
     const Dims &d = g.d;
     const uint32_t cta = blockIdx.x, ncta = gridDim.x;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 
-    StRing ring{full_bar, empty_bar, stage_tile, ssm + g.off_ring, g.nstages, g.stage_bytes};
+    // Register budget: 512 threads x 1 CTA caps a thread at 128 registers, and whatever the consumers' layer loop keeps live
+    // across a phase is paid for in every phase's peak (the prologue's staged words, the row loops' accumulators).  Values
+    // that are loop-invariant or rarely used are therefore re-read from shared memory (sg, s_*) where they are needed.
+    auto ring_of = [&]() { return StRing{full_bar, empty_bar, stage_tile, ssm + g.off_ring, g.nstages, g.stage_bytes}; };
     if (threadIdx.x == 0) {
         for (uint32_t s = 0; s < g.nstages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsWarps); stage_tile[s] = 0xffffffffu; }
         s_progress = 0; s_target = 0;
+        ss.step = 0; ss.pos = __ldcg(&g.st->pos);
+        ss.causal = __ldcg(&g.st->is_causal); ss.n_prompt = __ldcg(&g.st->n_prompt); ss.advance = __ldcg(&g.st->advance);
+        ss.pen = __ldcg(&g.st->penalty);
+        ss.tok = __ldcg(&g.st->use_token) ? __ldcg(&g.st->token) : __ldcg(g.ids + ss.pos);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     if (threadIdx.x < 5) {          // the rows this CTA owns of every kind (64-bit divisions: once, not once per phase)
@@ -1028,81 +1078,78 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
     }
     __syncthreads();
 
-    // step state (identical in every CTA; advanced locally)
-    uint32_t pos = __ldcg(&g.st->pos);
-    const uint32_t causal = __ldcg(&g.st->is_causal), n_prompt = __ldcg(&g.st->n_prompt), advance = __ldcg(&g.st->advance);
-    const float pen = __ldcg(&g.st->penalty);
-    uint32_t tok = __ldcg(&g.st->use_token) ? __ldcg(&g.st->token) : __ldcg(g.ids + pos);
-
     if (warp == kConsWarps) {
-        if (lane == 0) st_producer(g, ring, own, cta, &s_progress, pos, causal, advance);
+        if (lane == 0) st_producer(g, ring_of(), own, cta, &s_progress, ss.pos, ss.causal, ss.advance);
         return;
     }
 
-    unsigned char *act = ssm + g.off_act, *act_other = ssm + g.off_act2;
-    float *x_s = reinterpret_cast<float *>(ssm + g.off_xs);
-    float *attn_ws = reinterpret_cast<float *>(ssm + g.off_attn);
-    const uint32_t rep = cta % (uint32_t)kStRep;                       // the replica this CTA reads
-    const unsigned long long *rx = g.xv[0] + (size_t)rep * g.rs[0], *rxba = g.xv[1] + (size_t)rep * g.rs[1], *rhb = g.xv[2] + (size_t)rep * g.rs[2];
+    // the replica of a vector this CTA reads
+    auto xv_rep = [&](int i) -> const unsigned long long * { return g.xv[i] + (size_t)(blockIdx.x % (uint32_t)kStRep) * g.rs[i]; };
     StCursor cur{0u, 0u};
     uint32_t tcount = 0;                                                // tiles consumed so far (the producer counts the same way)
-    uint32_t ti = 0, tj = 0;
+    uint32_t act_flip = 0;                                              // consecutive phases alternate between the two operands
     // stamps (trace != nullptr: CTA 0 / thread 0, last step): [0..] after every phase; [1024..] inside layer L/2
-#define ST_TRACE() do { if (g.trace && cta == 0 && threadIdx.x == 0 && step + 1 == g.n_steps && ti < 1000) g.trace[ti++] = clock64(); } while (0)
-#define ST_STAMP() do { if (g.trace && cta == 0 && threadIdx.x == 0 && step + 1 == g.n_steps && l == d.L / 2 && tj < 60) g.trace[1024 + tj++] = clock64(); } while (0)
+    __shared__ uint32_t s_ti, s_tj;
+    if (st_tid() == 0) { s_ti = 0; s_tj = 0; }
+#define ST_TRACE() do { if (g.trace && cta == 0 && st_tid() == 0 && ss.step + 1 == g.n_steps && s_ti < 1000) g.trace[s_ti++] = clock64(); } while (0)
+#define ST_STAMP() do { if (g.trace && cta == 0 && st_tid() == 0 && ss.step + 1 == g.n_steps && l == d.L / 2 && s_tj < 60) g.trace[1024 + s_tj++] = clock64(); } while (0)
 
-    for (uint32_t step = 0; step < g.n_steps; step++) {
+    while (ss.step < g.n_steps) {
         ST_TRACE();
-        const uint32_t range = causal ? pos + 1u : d.max_seq;
-        uint32_t nsplit, chunk;
-        st_attn_plan(range, g.nsplit_max, g.chunk_target, nsplit, chunk);
+        if (st_tid() == 0) {       // read by the others after the barrier below
+            ss.range = ss.causal ? ss.pos + 1u : d.max_seq;
+            st_attn_plan(ss.range, g.nsplit_max, g.chunk_target, ss.nsplit, ss.chunk);
+        }
         // embedding row (infer.c:987-988) into shared memory; the rows this CTA owns in the residual phases start from it
-        embed_row<kConsThreads>(g.emb_w, g.emb_aux, x_s, tok, d);
-        cbar();
-        for (uint32_t i = threadIdx.x; i < own.rows[SK_O]; i += kConsThreads) xown[i] = x_s[own.row0[SK_O] + i];
-        // epochs of this token's exchanges: layer l publishes e0 + 5l + {1: q/k/v, 2: attention output, 3: x after O, 4: SwiGLU output, 5: x after W2}
-        const uint32_t e0 = g.epoch_base + step * 5u * d.L;
-
+        {
+            float *x_s = reinterpret_cast<float *>(ssm + g.off_xs);
+            embed_row<kConsThreads>(g.emb_w, g.emb_aux, x_s, ss.tok, d);
+            cbar();
+            for (uint32_t i = st_tid(); i < own.rows[SK_O]; i += kConsThreads) xown[i] = x_s[own.row0[SK_O] + i];
+        }
         // ---- layers 0..L-1: QKV | attention | O | W1,W3 | W2 ; pseudo-layer L: the classifier.  One call site per function. ----
 #pragma unroll 1
         for (uint32_t l = 0; l <= d.L; l++) {
             ST_STAMP();
-            const uint32_t el = e0 + 5u * l;
+            // epochs of this token's exchanges: layer l publishes el + {1: q/k/v, 2: attention output, 3: x after O, 4: SwiGLU output, 5: x after W2}
+            const uint32_t el = g.epoch_base + 5u * (ss.step * d.L + l);
 #pragma unroll 1
             for (uint32_t ph = 0; ph < 4; ph++) {
                 const bool cls = (l == d.L);
                 const uint32_t kid = cls ? (uint32_t)SK_CLS : ph;
                 const StKind &k = g.kind[kid];
-                const unsigned long long *xsrc = rx; const float *ssrc = nullptr; const float *gain = nullptr;
-                uint32_t epi, need = el, eout = 0;                        // x after the previous layer's W2 carries epoch e0 + 5(l-1) + 5 = el
+                const unsigned long long *xsrc = xv_rep(0); const float *ssrc = nullptr; const float *gain = nullptr;
+                uint32_t epi, need = el, eout = 0;                        // x after the previous layer's W2 carries epoch el(l-1) + 5 = el
                 if (cls) { gain = g.g_final; epi = EPI_CLS; }
-                else if (ph == SK_QKV) { if (l == 0) { xsrc = nullptr; ssrc = x_s; } gain = g.g_attn + (size_t)l * d.E; epi = EPI_QKV; eout = el + 1u; }
-                else if (ph == SK_O) { xsrc = rxba; need = el + 2u; epi = EPI_RESID; eout = el + 3u; }
+                else if (ph == SK_QKV) { if (l == 0) { xsrc = nullptr; ssrc = reinterpret_cast<const float *>(ssm + g.off_xs); } gain = g.g_attn + (size_t)l * d.E; epi = EPI_QKV; eout = el + 1u; }
+                else if (ph == SK_O) { xsrc = xv_rep(1); need = el + 2u; epi = EPI_RESID; eout = el + 3u; }
                 else if (ph == SK_W13) { need = el + 3u; gain = g.g_ffn + (size_t)l * d.E; epi = EPI_SWIGLU; eout = el + 4u; }
-                else { xsrc = rhb; need = el + 4u; epi = EPI_RESID; eout = el + 5u; }
-                unsigned long long *dbg = (g.trace && cta == 0 && step + 1 == g.n_steps && l == d.L / 2) ? g.trace + 1100 + 16 * ph : nullptr;
+                else { xsrc = xv_rep(2); need = el + 4u; epi = EPI_RESID; eout = el + 5u; }
+                unsigned long long *dbg = (g.trace && cta == 0 && ss.step + 1 == g.n_steps && l == d.L / 2) ? g.trace + 1100 + 16 * ph : nullptr;
                 if (g.ablate & 16u) need = kXwAny;
                 if (own.rows[kid]) {          // CTA-uniform: a CTA without rows of this kind neither reads the source nor publishes
-                    { unsigned char *t = act; act = act_other; act_other = t; }      // consecutive phases alternate between the two operands
+                    act_flip ^= 1u;
+                    unsigned char *act = ssm + (act_flip ? g.off_act2 : g.off_act);
                     st_prep<QUANT, LPG>(g, xsrc, ssrc, need, gain, k.n, act, ms.red, dbg);
                     ST_STAMP();
-                    st_consume<QUANT, LPG>(g, ring, cur, tcount, k, epi, l, own.row0[kid], own.rows[kid], eout, act, pos, pen, xown, ms, geo, kid, dbg);
+                    st_consume<QUANT, LPG>(g, ring_of(), cur, tcount, k, epi, l, own.row0[kid], own.rows[kid], eout, act, ss.pos, ss.pen, xown, ms, geo, kid, dbg);
                 } else {
                     ST_STAMP();
-                    if (cls && lane == 0) { ms.best_v[warp] = -FLT_MAX; ms.best_i[warp] = 0xffffffffu; }
+                    const uint32_t t = st_tid();
+                    if (cls && (t & 31u) == 0) { ms.best_v[t >> 5] = -FLT_MAX; ms.best_i[t >> 5] = 0xffffffffu; }
                 }
                 ST_STAMP();
                 ST_TRACE();
                 if (cls) break;
                 if (ph == SK_QKV) {
-                    st_attention<KVM>(g, ring, cur, tcount, l, cta, pos, range, nsplit, chunk, (g.ablate & 16u) ? kXwAny : el + 1u, el + 2u, attn_ws, dbg ? g.trace + 1100 + 64 : nullptr);
+                    st_attention<KVM>(g, ring_of(), cur, tcount, l, cta, ss.pos, ss.range, ss.nsplit, ss.chunk, (g.ablate & 16u) ? kXwAny : el + 1u, el + 2u, reinterpret_cast<float *>(ssm + g.off_attn), dbg ? g.trace + 1100 + 64 : nullptr);
                     ST_STAMP();
                     ST_TRACE();
                 }
             }
         }
         cbar();
-        if (threadIdx.x == 0) {
+        if (st_tid() == 0) {
             float bv = ms.best_v[0]; uint32_t bi = ms.best_i[0];
             for (int w = 1; w < kConsWarps; w++)
                 if (ms.best_i[w] != 0xffffffffu && (bi == 0xffffffffu || ms.best_v[w] > bv || (ms.best_v[w] == bv && ms.best_i[w] < bi))) { bv = ms.best_v[w]; bi = ms.best_i[w]; }
@@ -1113,7 +1160,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
         // ---- every CTA picks the token from the per-CTA partials (no second barrier) and advances its copy of the state ----
         {
             float bv = -FLT_MAX; uint32_t bi = 0xffffffffu;
-            for (uint32_t c2 = threadIdx.x; c2 < ncta; c2 += kConsThreads) {
+            for (uint32_t c2 = st_tid(); c2 < ncta; c2 += kConsThreads) {
                 const float v = __ldcg(g.cls_val + c2); const uint32_t i = __ldcg(g.cls_idx + c2);
                 if (i != 0xffffffffu && (bi == 0xffffffffu || v > bv || (v == bv && i < bi))) { bv = v; bi = i; }
             }
@@ -1122,26 +1169,31 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
                 const float ov = __shfl_xor_sync(0xffffffffu, bv, o); const uint32_t oi = __shfl_xor_sync(0xffffffffu, bi, o);
                 if (oi != 0xffffffffu && (bi == 0xffffffffu || ov > bv || (ov == bv && oi < bi))) { bv = ov; bi = oi; }
             }
-            if (lane == 0) { ms.best_v[warp] = bv; ms.best_i[warp] = bi; }
+            const uint32_t t = st_tid();
+            if ((t & 31u) == 0) { ms.best_v[t >> 5] = bv; ms.best_i[t >> 5] = bi; }
             cbar();
-            bv = -FLT_MAX; bi = 0xffffffffu;
+            if (st_tid() == 0) {
+                bv = -FLT_MAX; bi = 0xffffffffu;
 #pragma unroll 1
-            for (int w = 0; w < kConsWarps; w++)
-                if (ms.best_i[w] != 0xffffffffu && (bi == 0xffffffffu || ms.best_v[w] > bv || (ms.best_v[w] == bv && ms.best_i[w] < bi))) { bv = ms.best_v[w]; bi = ms.best_i[w]; }
-            if (bi == 0xffffffffu) bi = 0;       // all-NaN row: the reference's argmax returns index 0
-            uint32_t nxt = bi;
-            if (advance) {
-                const bool forced = (pos + 1 < n_prompt);            // infer.c:1250 is_prefilling
-                if (forced) nxt = __ldcg(g.ids + pos + 1);
-                if (cta == 0 && threadIdx.x == 0) {
-                    g.seen[tok] = 1;                                 // ids[0..pos] are "seen" for step pos+1
-                    if (!forced) g.ids[pos + 1] = bi;
-                    g.st->pos = pos + 1;
-                    g.st->next_token = nxt;
+                for (int w = 0; w < kConsWarps; w++)
+                    if (ms.best_i[w] != 0xffffffffu && (bi == 0xffffffffu || ms.best_v[w] > bv || (ms.best_v[w] == bv && ms.best_i[w] < bi))) { bv = ms.best_v[w]; bi = ms.best_i[w]; }
+                if (bi == 0xffffffffu) bi = 0;       // all-NaN row: the reference's argmax returns index 0
+                const uint32_t pos = ss.pos, tok = ss.tok;
+                uint32_t nxt = bi;
+                if (ss.advance) {
+                    const bool forced = (pos + 1 < ss.n_prompt);     // infer.c:1250 is_prefilling
+                    if (forced) nxt = __ldcg(g.ids + pos + 1);
+                    if (cta == 0) {
+                        g.seen[tok] = 1;                             // ids[0..pos] are "seen" for step pos+1
+                        if (!forced) g.ids[pos + 1] = bi;
+                        g.st->pos = pos + 1;
+                        g.st->next_token = nxt;
+                    }
+                    ss.tok = nxt; ss.pos = pos + 1;
+                } else if (cta == 0) {
+                    g.st->next_token = bi;
                 }
-                tok = nxt; pos = pos + 1;
-            } else if (cta == 0 && threadIdx.x == 0) {
-                g.st->next_token = bi;
+                ss.step = ss.step + 1u;
             }
             cbar();
         }
