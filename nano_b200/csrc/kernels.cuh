@@ -327,12 +327,13 @@ __device__ void prep_f32(const float *src, const float *__restrict__ gain, int n
 
 // (int8) round(x / scale) of tensor.c:40-42, bit-exact with a fast path: q = x * (1/scale) is within ~4e-5 of the
 // correctly rounded quotient for |q| <= 127, so unless q sits within 1e-3 of a .5 boundary the rounded integer is
-// unambiguous; the rare boundary case takes the IEEE division + roundf path.
+// unambiguous; the rare boundary case takes the IEEE division + roundf path.  A group with amax below ~3.74e-37 has a
+// scale under 1/FLT_MAX, so rinv = +inf and frac = NaN: the negated test sends that to the exact path as well.
 static __device__ __noinline__ int q80_code_slow(float v, float sc) { return (int)roundf(__fdiv_rn(v, sc)); }   // rare: kept out of line
 __device__ __forceinline__ int q80_code(float v, float sc, float rinv) {
     const float q = v * rinv;
     const float a = fabsf(q), fl = floorf(a), frac = a - fl;
-    if (fabsf(frac - 0.5f) < 1e-3f) return q80_code_slow(v, sc);
+    if (!(fabsf(frac - 0.5f) >= 1e-3f)) return q80_code_slow(v, sc);
     const int c = (int)fl + (frac > 0.5f ? 1 : 0);
     return q < 0.0f ? -c : c;
 }

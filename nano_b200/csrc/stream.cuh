@@ -404,14 +404,16 @@ __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long
                     if (on) {
                         uint32_t pk = 0;
                         if (sc != 0.0f && !(g.ablate & 1u)) {
-                            int cq[4]; bool tie = false;
+                            int cq[4]; bool tie = rinv == 0.0f;
 #pragma unroll
                             for (int u = 0; u < 4; u++) {
                                 const float q = av[u] * rinv, aq = fabsf(q);
                                 const float rr = aq + 12582912.0f;                 // 1.5 * 2^23: the integer nearest to aq sits in the mantissa
                                 const float cf = rr - 12582912.0f;
                                 const int c = __float_as_int(rr) - 0x4b400000;
-                                tie = tie || fabsf(aq - cf) > 0.499f;
+                                // rinv = inf (amax < ~3.74e-37) makes this NaN and rinv = 0 (__fdividef, amax > 2^126) makes
+                                // every code 0: both take the exact path
+                                tie = tie || !(fabsf(aq - cf) <= 0.499f);
                                 cq[u] = q < 0.0f ? -c : c;
                             }
                             pk = ((uint32_t)cq[0] & 0xffu) | (((uint32_t)cq[1] & 0xffu) << 8) | (((uint32_t)cq[2] & 0xffu) << 16) | (((uint32_t)cq[3] & 0xffu) << 24);

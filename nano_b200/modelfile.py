@@ -95,6 +95,20 @@ PRESETS: Dict[str, ModelSpec] = {
     # long-context shapes (2 layers of the Nano-168M / Qwen3-0.6B layer shape): attention with many splits and segments
     "long-nano": ModelSpec("long-nano", ARCH_NANO, 4096, 2048, 2, 768, 16, 8, 2048),
     "long-qwen3": ModelSpec("long-qwen3", ARCH_QWEN3, 4096, 4096, 2, 1024, 16, 8, 3072, 128),
+    # 2-layer shapes that select every instantiation of the streaming kernel and of the split-KV attention kernel
+    # (KVM = n_head / n_kv_head in {1, 2, 4}) and every activation-prologue width class (tests/test_gpu_stream_matrix.py)
+    "kvm1-nano": ModelSpec("kvm1-nano", ARCH_NANO, 2048, 2048, 2, 512, 8, 8, 1024),
+    "kvm4-qwen3-hd128": ModelSpec("kvm4-qwen3-hd128", ARCH_QWEN3, 2048, 4096, 2, 1024, 16, 4, 2048, 128),
+    "kvm4-qwen3-hd64": ModelSpec("kvm4-qwen3-hd64", ARCH_QWEN3, 2048, 4096, 2, 512, 8, 2, 1024, 64),
+    "hd52-nano": ModelSpec("hd52-nano", ARCH_NANO, 2048, 1024, 2, 208, 4, 2, 520),          # hd % 16 != 0, partial prologue slots
+    "qwen3-4b-2l": ModelSpec("qwen3-4b-2l", ARCH_QWEN3, 256, 4096, 2, 2560, 32, 8, 9728, 128),   # Qwen3-4B layer shape
+    "ffn3840-nano": ModelSpec("ffn3840-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 3840),      # one full poll batch
+    "ffn3968-nano": ModelSpec("ffn3968-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 3968),      # one slot into the second batch
+    "ffn4096-nano": ModelSpec("ffn4096-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 4096),      # Q4K: second warp slot
+    "ffn7680-nano": ModelSpec("ffn7680-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 7680),      # Q4K: st_prep_max_n
+    "ffn7936-nano": ModelSpec("ffn7936-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 7936),      # Q4K: one block past it
+    "ffn11520-nano": ModelSpec("ffn11520-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 11520),   # Q80 / F32: st_prep_max_n
+    "ffn11648-nano": ModelSpec("ffn11648-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 11648),   # Q80 / F32: one group past it
 }
 
 

@@ -16,6 +16,8 @@ Run in the build container (needs /root/reference):   python tests/golden/make_g
   export_nano.npz      the reference exporter (export.py) run on the seeded tiny GPT of nano_export_weights(): SHA-256 digests
                        of its F32 / Q80 / LoRA files, the model's RoPE tables and its PyTorch logits over 12 teacher-forced
                        positions:  python tests/golden/make_golden.py --export
+  reference_noise_floor.json  max |fast build - strict build| of the reference's logits per quantised test file; the floors of
+                       the stream-matrix files alone:  python tests/golden/make_golden.py --floors
 """
 import ctypes as C
 import hashlib
@@ -145,6 +147,38 @@ def export_digests(reference_root: str = os.path.dirname(ob.REFERENCE_SRC)):
     print("export digests written")
 
 
+# the quantised files of tests/test_gpu_stream_matrix.py
+MATRIX_FLOOR_CASES = ([(n, q, g) for n in ("kvm1-nano", "kvm4-qwen3-hd128", "kvm4-qwen3-hd64", "ffn3840-nano")
+                       for q, g in ((mf.QUANT_Q80, 128), (mf.QUANT_Q80, 64), (mf.QUANT_Q4K, 128))] +
+                      [("qwen3-4b-2l", mf.QUANT_Q80, 128), ("ffn3968-nano", mf.QUANT_Q80, 128), ("ffn3968-nano", mf.QUANT_Q80, 64),
+                       ("ffn4096-nano", mf.QUANT_Q4K, 128), ("ffn4096-nano", mf.QUANT_Q80, 64), ("ffn7680-nano", mf.QUANT_Q4K, 128),
+                       ("ffn7680-nano", mf.QUANT_Q80, 128), ("ffn11520-nano", mf.QUANT_Q80, 128), ("ffn11520-nano", mf.QUANT_Q80, 64),
+                       ("ffn7936-nano", mf.QUANT_Q4K, 128), ("ffn7936-nano", mf.QUANT_Q80, 128), ("ffn11648-nano", mf.QUANT_Q80, 128)])
+
+
+def noise_floors(cases, S=40):
+    """Noise floor of the reference itself: max |logit(fast build) - logit(strict build)| of the SAME source on the SAME
+    file (SURVEY finding 11), over S teacher-forced positions.  The fast-mode GPU tolerance is max(north-star tolerance,
+    1.5 x this floor)."""
+    floors = {}
+    for name, quant, gs in cases:
+        spec = mf.PRESETS[name]
+        path = mf.cached_model(spec, quant, gs)
+        a = ob.RefEngine(path, S, "strict")
+        toks = mf.teacher_tokens(S, spec.vocab)
+        strict = [a.forward(toks[p], p) for p in range(S)]
+        worst = 0.0
+        for fl in ("fast_v3", "fast_v4"):
+            b = ob.RefEngine(path, S, fl)
+            for p in range(S):
+                worst = max(worst, float(np.abs(b.forward(toks[p], p) - strict[p]).max()))
+            b.close()
+        a.close()
+        floors[f"{name}_{quant:02x}_{gs}"] = worst
+        print(name, f"{quant:#x}", gs, worst)
+    return floors
+
+
 def reference_digests():
     """reference_outputs.json from the unmodified strict reference (oracle/_ref)."""
     ob.build()
@@ -235,24 +269,8 @@ def main():
         r.close()
     np.savez_compressed(os.path.join(HERE, "lora_logits.npz"), **lora_out)
 
-    # Noise floor of the reference itself: max |logit(fast build) - logit(strict build)| of the SAME source on the
-    # SAME file (SURVEY finding 11).  The fast-mode GPU tolerance is max(north-star tolerance, 1.5 x this floor).
-    floors = {}
-    S = 40
-    for name, quant, gs in TOY_CONFIGS + [("mini-qwen3", mf.QUANT_Q80, 128), ("mini-nano", mf.QUANT_Q80, 128), ("mini-nano", mf.QUANT_Q4K, 128)]:
-        spec = mf.PRESETS[name]
-        path = mf.cached_model(spec, quant, gs)
-        a = ob.RefEngine(path, S, "strict")
-        toks = mf.teacher_tokens(S, spec.vocab)
-        strict = [a.forward(toks[p], p) for p in range(S)]
-        worst = 0.0
-        for fl in ("fast_v3", "fast_v4"):
-            b = ob.RefEngine(path, S, fl)
-            for p in range(S):
-                worst = max(worst, float(np.abs(b.forward(toks[p], p) - strict[p]).max()))
-            b.close()
-        a.close()
-        floors[f"{name}_{quant:02x}_{gs}"] = worst
+    floors = noise_floors(TOY_CONFIGS + [("mini-qwen3", mf.QUANT_Q80, 128), ("mini-nano", mf.QUANT_Q80, 128), ("mini-nano", mf.QUANT_Q4K, 128)]
+                          + MATRIX_FLOOR_CASES)
     json.dump(floors, open(os.path.join(HERE, "reference_noise_floor.json"), "w"), indent=1)
     print("floors", floors)
 
@@ -282,5 +300,11 @@ if __name__ == "__main__":
         reference_digests()
     elif "--export" in sys.argv:
         export_digests()
+    elif "--floors" in sys.argv:           # add the stream-matrix floors to the committed ones
+        ob.build()
+        path = os.path.join(HERE, "reference_noise_floor.json")
+        floors = json.load(open(path))
+        floors.update(noise_floors(MATRIX_FLOOR_CASES))
+        json.dump(floors, open(path, "w"), indent=1)
     else:
         main()

@@ -77,6 +77,8 @@ def test_teacher_forced_logits_fast_mode(name, quant, gs, path_flags, monkeypatc
     if path_flags == -1:      # the streaming kernel's throughput mode (one warp per tile), which toy shapes would not reach by themselves
         monkeypatch.setenv("NB200_OWNED_ROWS", "2"); path_flags = 0
     eng = E.Engine(path, S, flags=path_flags); o = ob.NanoOracle(path, S)
+    # setup_stream declines a shape without an error: a case must fail, not quietly test the other path
+    assert eng.path.startswith("multi-kernel" if path_flags == E.FLAG_NO_STREAM else "streaming"), eng.path
     toks = mf.teacher_tokens(S, spec.vocab)
     floor = reference_noise_floor(name, quant, gs, path, S)
     limit = max(TOL[quant], 1.5 * floor)

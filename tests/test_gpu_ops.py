@@ -92,6 +92,79 @@ def test_q80_quantize_half_ties():
     assert_bits_equal(q, wq, "codes")
 
 
+def q80_edge_vector(gs):
+    """One group per edge case: a scale reciprocal that overflows (amax just below ~3.74e-37) or just does not, subnormal
+    amax, signed zeros only, a single nonzero element, a negative maximum, exact .5 ties at scales other than 1, values
+    5e-5 and 2e-3 from a tie, amax near FLT_MAX, and normal groups in between (mixed tiny and normal groups in one vector)."""
+    rng = np.random.default_rng(gs)
+    f = np.float32
+    groups = []
+
+    def grp(amax, sign=1.0):
+        g = (rng.uniform(-1, 1, gs).astype(np.float32) * f(amax)).astype(np.float32)
+        g[rng.integers(gs)] = f(sign) * f(amax)
+        return g
+    for amax in (3.6e-37, 3.7e-37, 3.73e-37, 3.75e-37, 3.8e-37, 1e-36, 1.17549435e-38):   # around the rinv overflow, FLT_MIN
+        groups += [grp(amax), rng.standard_normal(gs).astype(np.float32)]
+    for amax in (1e-40, 1.4e-45 * 5, 1.4e-45):                                              # subnormal amax
+        groups.append(grp(amax))
+    z = np.zeros(gs, np.float32); z[1::2] = -0.0
+    groups.append(z)                                                                        # +-0 only
+    one = np.zeros(gs, np.float32); one[gs // 3] = f(-2.5e-3)
+    groups.append(one)                                                                      # a single nonzero element
+    groups.append(grp(7.25, -1.0))                                                          # negative maximum
+    for sc in (f(0.375), f(3.0517578125e-05), f(96.0)):                                     # exact ties at scale sc
+        t = np.zeros(gs, np.float32)
+        t[0] = f(127) * sc
+        k = np.arange(1, gs) % 126
+        t[1:] = ((k + f(0.5)) * sc * np.where(np.arange(1, gs) % 2, 1, -1)).astype(np.float32)
+        groups.append(t)
+        # x / scale 5e-5 from a tie (inside the fast path's 1e-3 fallback window) and 2e-3 from one (just outside it)
+        nt = t.copy()
+        off = np.array([5e-5, -5e-5, 2e-3, -2e-3], np.float32)[np.arange(1, gs) % 4]
+        nt[1:] = ((k + f(0.5) + off) * sc * np.where(np.arange(1, gs) % 2, 1, -1)).astype(np.float32)
+        groups.append(nt)
+    groups += [grp(3.4e38), grp(3.3e38, -1.0), grp(1.7e38), grp(9e37)]                       # amax near FLT_MAX, above 2^126
+    return np.concatenate(groups).astype(np.float32)
+
+
+@pytest.mark.parametrize("gs", [32, 64, 128, 256])
+def test_q80_quantize_edges_bit_exact(gs):
+    """Codes and scales bit-identical to tensor.c:21-46 on groups at the edges of the float range.  With amax < ~3.74e-37
+    the scale amax/127 is below 1/FLT_MAX and its reciprocal overflows: the fast path must fall back to the division."""
+    x = q80_edge_vector(gs)
+    q, s = E.op_q80_quantize(x, gs)
+    wq, ws = o_q80_quant(x, gs)
+    assert_bits_equal(s, ws, "scales")
+    bad = np.nonzero(q != wq)[0]
+    assert bad.size == 0, f"{bad.size} codes differ; first at {bad[:4]} (group {bad[0] // gs}): {q[bad[:4]]} vs {wq[bad[:4]]}"
+
+
+def q4k_edge_vector():
+    """Constant blocks (positive, negative, zero), tiny and huge blocks, all-negative and all-positive blocks, one
+    nonzero element, and a block that mixes the extremes group by group."""
+    rng = np.random.default_rng(11)
+    f = np.float32
+    blocks = [np.full(256, f(0.75)), np.full(256, f(-1.25)), np.zeros(256, np.float32),
+              rng.standard_normal(256).astype(np.float32) * f(1e-38), rng.standard_normal(256).astype(np.float32) * f(1e-42),
+              rng.standard_normal(256).astype(np.float32) * f(1e36), rng.uniform(-1.5e38, 1.5e38, 256).astype(np.float32),
+              -np.abs(rng.standard_normal(256)).astype(np.float32) - f(0.5), np.abs(rng.standard_normal(256)).astype(np.float32) + f(0.5)]
+    one = np.zeros(256, np.float32); one[77] = f(-3.0)
+    blocks.append(one)
+    mix = rng.standard_normal(256).astype(np.float32)
+    mix[0:32] *= f(1e-39); mix[32:64] *= f(1e30); mix[64:96] = f(2.0); mix[96:128] = -np.abs(mix[96:128])
+    blocks.append(mix)
+    return np.concatenate(blocks).astype(np.float32)
+
+
+def test_q4k_quantize_edges_bit_exact():
+    x = q4k_edge_vector()
+    assert_bits_equal(E.op_q4k_quantize(x), o_q4k_quant(x), "q4k activation blocks")
+    want = np.zeros((x.size // 256) * 160, np.uint8)
+    oracle().nor_q4k_quantize_rows(want.ctypes.data_as(ob.u8p), x.ctypes.data_as(ob.f32p), 1, x.size)
+    assert_bits_equal(E.op_q4k_quantize_blocks(x), want, "q4k tensor blocks")
+
+
 @pytest.mark.parametrize("n,d,gs", [(256, 7, 64), (256, 33, 32), (768, 64, 128), (1024, 1000, 128), (1024, 130, 64),
                                     (3072, 257, 128), (2048, 96, 256), (2560, 50, 128), (9728, 40, 128)])
 def test_q80_matvec_bit_exact(n, d, gs):
