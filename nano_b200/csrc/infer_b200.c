@@ -277,6 +277,11 @@ static int sample_nucleus(Nano_Context *ctx, float *prob, int n, float top_p, Pr
         for (int i = 0; i < 6; i++) t[i] = (m > i) ? (uint32_t)pi[i].index : 0u;
         ctx->observation(o, ctx->observation_env);
     }
+    if (m == 0) {               /* no candidate (the reference reads pi[-1]): first-max argmax, as the device sampler does */
+        int best = 0;
+        for (int i = 1; i < n; i++) if (prob[i] > prob[best]) best = i;
+        return best;
+    }
     const float r = coin * cum;
     float cdf = 0.0f;
     for (int i = 0; i <= last; i++) { cdf += pi[i].prob; if (r < cdf) return pi[i].index; }

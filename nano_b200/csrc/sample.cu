@@ -20,13 +20,14 @@ namespace nb {
 constexpr int kSampThreads = 1024;
 constexpr int kSampChunk = 4096;       // floats staged in shared memory per step of a sequential scan
 
-// pass 1: y = logit / T, max; p = expf(y - max); sequential sum; p /= sum; key = p >= cutoff ? p : -1; n0 = #candidates
+// pass 1: y = logit / T, max; p = expf(y - max); sequential sum; p /= sum; key = p >= cutoff ? p : -1; out[7] = n0 = #candidates,
+// out[8] = the first index of the largest p
 __global__ void __launch_bounds__(kSampThreads) k_sample_prepare(const float *__restrict__ logits, uint32_t V, float temperature, float top_p,
                                                                  float *keys, uint32_t *vals, uint32_t *out) {
     __shared__ float red[32];
     __shared__ float chunk[kSampChunk];
     __shared__ float s_total;
-    __shared__ uint32_t s_cnt;
+    __shared__ uint32_t s_cnt, s_best[32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float mx = -FLT_MAX;
     for (uint32_t i = threadIdx.x; i < V; i += kSampThreads) {
@@ -54,18 +55,31 @@ __global__ void __launch_bounds__(kSampThreads) k_sample_prepare(const float *__
     total = s_total;
     const float cutoff = __fdiv_rn(__fsub_rn(1.0f, top_p), (float)(int)(V - 1));        // infer.c:1064
     uint32_t cnt = 0;
+    float bp = -1.0f;                 // first-max argmax of the probabilities: the pick when no candidate passes the cutoff
+    uint32_t bi = 0;
     for (uint32_t i = threadIdx.x; i < V; i += kSampThreads) {
         const float p = __fdiv_rn(keys[i], total);                   // infer.c:632
         const bool in = p >= cutoff;
         keys[i] = in ? p : -1.0f;
         vals[i] = i;
         cnt += in ? 1u : 0u;
+        if (p > bp) { bp = p; bi = i; }                              // ascending i per thread: the thread's first max
     }
-    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    for (int o = 16; o > 0; o >>= 1) {
+        cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        const float op = __shfl_xor_sync(0xffffffffu, bp, o);
+        const uint32_t oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (op > bp || (op == bp && oi < bi)) { bp = op; bi = oi; }
+    }
+    if (lane == 0) { red[warp] = bp; s_best[warp] = bi; }
     if (lane == 0 && cnt) atomicAdd(&s_cnt, cnt);
-    (void)warp;
     __syncthreads();
-    if (threadIdx.x == 0) out[7] = s_cnt;
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < kSampThreads / 32; w++)
+            if (red[w] > bp || (red[w] == bp && s_best[w] < bi)) { bp = red[w]; bi = s_best[w]; }
+        out[7] = s_cnt;
+        out[8] = bi;
+    }
 }
 
 // pass 2 (after the sort): cumulative sum to top_p, then the CDF walk (infer.c:1076-1106), both sequential
@@ -75,6 +89,17 @@ __global__ void __launch_bounds__(256) k_sample_pick(const float *__restrict__ k
     __shared__ uint32_t s_stop, s_last;
     __shared__ float s_cum;
     const uint32_t n0 = out[7];
+    if (n0 == 0) {
+        // No probability reaches the cutoff (top_p < 1/V over a near-flat distribution).  The reference then reads
+        // probindex[-1] (undefined); this sampler returns the first-max argmax of the probabilities and six zero ids.
+        if (threadIdx.x == 0) {
+            const uint32_t tok = out[8];
+            out[0] = tok;
+            for (uint32_t i = 0; i < 6; i++) out[1 + i] = 0u;
+            if (st) st->next_token = tok;
+        }
+        return;
+    }
     if (threadIdx.x == 0) { s_stop = 0; s_last = n0 - 1; s_cum = 0.0f; }
     __syncthreads();
     float cum = 0.0f;
@@ -93,6 +118,7 @@ __global__ void __launch_bounds__(256) k_sample_pick(const float *__restrict__ k
     }
     const uint32_t last = s_last;
     const float r = __fmul_rn(coin, s_cum);
+    __syncthreads();                  // every warp has read s_stop in its loop test before it is cleared for the CDF walk
     if (threadIdx.x == 0) s_stop = 0;
     __syncthreads();
     float cdf = 0.0f;
@@ -118,6 +144,22 @@ __global__ void __launch_bounds__(256) k_sample_pick(const float *__restrict__ k
     }
 }
 
+// The workspace: keys and values in and out (V words each, 256-byte aligned), the sort's temporary storage, then the result
+// words {token, top-6 ids, n0, first-max index} in the last 256 bytes.
+struct SampleWorkspace {
+    float *keys_in, *keys_out;
+    uint32_t *vals_in, *vals_out;
+    void *tmp;
+    uint32_t *out;
+};
+
+static inline SampleWorkspace sample_workspace(void *workspace, uint32_t V, size_t cub_bytes) {
+    const size_t a = ((size_t)V * 4 + 255) & ~(size_t)255;
+    unsigned char *w = static_cast<unsigned char *>(workspace);
+    return {reinterpret_cast<float *>(w), reinterpret_cast<float *>(w + a), reinterpret_cast<uint32_t *>(w + 2 * a),
+            reinterpret_cast<uint32_t *>(w + 3 * a), w + 4 * a, reinterpret_cast<uint32_t *>(w + 4 * a + ((cub_bytes + 255) & ~(size_t)255))};
+}
+
 size_t sample_workspace_bytes(uint32_t V, size_t *cub_bytes) {
     size_t tmp = 0;
     cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp, (const float *)nullptr, (float *)nullptr, (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)V);
@@ -128,20 +170,15 @@ size_t sample_workspace_bytes(uint32_t V, size_t *cub_bytes) {
 
 cudaError_t sample_top_p_launch(void *workspace, size_t cub_bytes, const float *logits, uint32_t V, float temperature, float top_p, float coin,
                                 DevState *st, uint32_t **out_dev, cudaStream_t stream) {
-    const size_t a = ((size_t)V * 4 + 255) & ~(size_t)255;
-    unsigned char *w = static_cast<unsigned char *>(workspace);
-    float *keys_in = reinterpret_cast<float *>(w), *keys_out = reinterpret_cast<float *>(w + a);
-    uint32_t *vals_in = reinterpret_cast<uint32_t *>(w + 2 * a), *vals_out = reinterpret_cast<uint32_t *>(w + 3 * a);
-    void *tmp = w + 4 * a;
-    uint32_t *out = reinterpret_cast<uint32_t *>(w + 4 * a + ((cub_bytes + 255) & ~(size_t)255));
-    k_sample_prepare<<<1, kSampThreads, 0, stream>>>(logits, V, temperature, top_p, keys_in, vals_in, out);
+    const SampleWorkspace w = sample_workspace(workspace, V, cub_bytes);
+    k_sample_prepare<<<1, kSampThreads, 0, stream>>>(logits, V, temperature, top_p, w.keys_in, w.vals_in, w.out);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     size_t tb = cub_bytes;
-    e = cub::DeviceRadixSort::SortPairsDescending(tmp, tb, keys_in, keys_out, vals_in, vals_out, (int)V, 0, 32, stream);
+    e = cub::DeviceRadixSort::SortPairsDescending(w.tmp, tb, w.keys_in, w.keys_out, w.vals_in, w.vals_out, (int)V, 0, 32, stream);
     if (e != cudaSuccess) return e;
-    k_sample_pick<<<1, 256, 0, stream>>>(keys_out, vals_out, top_p, coin, out, st);
-    *out_dev = out;
+    k_sample_pick<<<1, 256, 0, stream>>>(w.keys_out, w.vals_out, top_p, coin, w.out, st);
+    *out_dev = w.out;
     return cudaGetLastError();
 }
 

@@ -109,6 +109,11 @@ PRESETS: Dict[str, ModelSpec] = {
     "ffn7936-nano": ModelSpec("ffn7936-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 7936),      # Q4K: one block past it
     "ffn11520-nano": ModelSpec("ffn11520-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 11520),   # Q80 / F32: st_prep_max_n
     "ffn11648-nano": ModelSpec("ffn11648-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 11648),   # Q80 / F32: one group past it
+    # 2-layer models with the real vocabularies (Nano-168M, Qwen3): the sampler's scans over many 4096-entry chunks
+    # (tests/test_gpu_sampler.py, tests/test_gpu_shim.py)
+    "v16k-nano": ModelSpec("v16k-nano", ARCH_NANO, 128, 16384, 2, 256, 4, 2, 512),
+    "v152k-qwen3": ModelSpec("v152k-qwen3", ARCH_QWEN3, 128, 151936, 2, 256, 4, 2, 512, 64),
+    "v152k-qwen3-untied": ModelSpec("v152k-qwen3-untied", ARCH_QWEN3, 128, 151936, 2, 256, 4, 2, 512, 64, 0),
 }
 
 

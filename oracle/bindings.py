@@ -149,6 +149,38 @@ class NanoOracle:
         return buf
 
 
+def sample_top_p(logits, temperature: float, top_p: float, coin: float, sorted_out: bool = False):
+    """nor_sample_top_p: (id, six observed ids, n0, last) and, with sorted_out, the n0 sorted (probabilities, indices).
+    last is -1 when n0 = 0."""
+    lg = np.ascontiguousarray(logits, np.float32)
+    V = lg.size
+    out = np.zeros(9, np.uint32)
+    sp = np.zeros(V, np.float32) if sorted_out else None
+    si = np.zeros(V, np.uint32) if sorted_out else None
+    f = NanoOracle.lib().nor_sample_top_p          # bound here: NanoOracle.lib() stays usable with an older build
+    f.argtypes = [f32p, C.c_uint32, C.c_float, C.c_float, C.c_float, u32p, f32p, u32p]
+    f.restype = None
+    f(_ptr(lg, f32p), V, temperature, top_p, coin, _ptr(out, u32p),
+      None if sp is None else _ptr(sp, f32p), None if si is None else _ptr(si, u32p))
+    res = (int(out[0]), [int(t) for t in out[1:7]], int(out[7]), int(out[8].view(np.int32)))
+    if sorted_out:
+        return res + (sp[:out[7]], si[:out[7]])
+    return res
+
+
+def random_f32(state: int):
+    """utils.c:959-970: xorshift64* step, top 24 bits / 2^24.  Returns (coin, new state)."""
+    m = (1 << 64) - 1
+    state ^= state >> 12
+    state ^= (state << 25) & m
+    state ^= state >> 27
+    return np.float32(((state * 0x2545F4914F6CDD1D) & m) >> 40) / np.float32(16777216.0), state
+
+
+class ProbIndex(C.Structure):          # infer.h:210-213
+    _fields_ = [("prob", C.c_float), ("index", C.c_int)]
+
+
 class Q80Tensor(C.Structure):          # tensor.h:84-90
     _fields_ = [("q", i8p), ("s", f32p)]
 
@@ -187,6 +219,8 @@ class RefEngine:
             L.orh_sort_model.argtypes = [u32p]
             L.orh_abi_layout.restype = C.c_uint32
             L.orh_abi_layout.argtypes = [u32p, C.c_uint32]
+            L.sample_top_p.restype = C.c_int
+            L.sample_top_p.argtypes = [C.c_void_p, f32p, C.c_int, C.c_float, C.c_void_p, C.c_float]
             L.seq2seq.argtypes = [C.c_void_p, C.c_wchar_p, C.c_wchar_p, C.c_uint32]
             # raw reference ops (non-static symbols of infer.c / tensor.c)
             L.rmsnorm.argtypes = [f32p, f32p, f32p, C.c_int]
@@ -262,6 +296,19 @@ class RefEngine:
         out = C.create_unicode_buffer(n + 8)
         self.L.seq2seq(self.h, text, out, n)
         return out.value
+
+
+def ref_last_sample(flavour: str = "strict"):
+    """orh_last_sample of the harness (the six ids of the last sampling observation), or None when the harness in
+    oracle/_ref was built before it existed.  Bound on demand, so that such a harness still serves every other test."""
+    L = RefEngine.lib(flavour)
+    try:
+        f = L.orh_last_sample
+    except AttributeError:
+        return None
+    f.argtypes = [u32p]
+    f.restype = None
+    return f
 
 
 def sort_model_bytes(flavour: str = "strict") -> bytes:

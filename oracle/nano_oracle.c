@@ -582,6 +582,70 @@ uint32_t nor_next_greedy(NorModel *m, const uint32_t *ids, uint32_t pos, int pre
 }
 
 /* ------------------------------------------------------------------------------------------ */
+/* Temperature / top-p sampling (infer.c:1174-1189, sample_top_p :1062-1109)                    */
+/* ------------------------------------------------------------------------------------------ */
+typedef struct { float prob; uint32_t index; } NorProbIndex;
+
+/* infer.c:1053-1059 */
+static int nor_prob_desc(const NorProbIndex *a, const NorProbIndex *b) {
+    if (a->prob > b->prob) return -1;
+    if (a->prob < b->prob) return 1;
+    return 0;
+}
+
+/* stable merge sort by nor_prob_desc: the order glibc's (merge-sort) qsort gives the reference */
+static void nor_sort_stable(NorProbIndex *a, NorProbIndex *tmp, uint32_t n) {
+    for (uint32_t w = 1; w < n; w *= 2) {
+        for (uint32_t lo = 0; lo < n; lo += 2 * w) {
+            const uint32_t mid = lo + w < n ? lo + w : n, hi = lo + 2 * w < n ? lo + 2 * w : n;
+            uint32_t i = lo, j = mid, k = lo;
+            while (i < mid && j < hi) tmp[k++] = nor_prob_desc(&a[j], &a[i]) < 0 ? a[j++] : a[i++];
+            while (i < mid) tmp[k++] = a[i++];
+            while (j < hi) tmp[k++] = a[j++];
+        }
+        memcpy(a, tmp, (size_t)n * sizeof *a);
+    }
+}
+
+/* One sampling step on `logits` [V] (penalty already applied; not modified).
+ * out[0] = id, out[1..6] = the observation hook's six ids (0 where n0 <= i), out[7] = n0, out[8] = last (0xffffffff if n0 = 0).
+ * sorted_p / sorted_i (optional, V entries): the n0 candidates in sorted order.
+ * n0 = 0 (no probability reaches the cutoff) is undefined in the reference (probindex[-1]); here, as in the engine, the id is
+ * the first-max argmax of the probabilities and the six ids are 0. */
+void nor_sample_top_p(const float *logits, uint32_t V, float temperature, float top_p, float coin, uint32_t out[9],
+                      float *sorted_p, uint32_t *sorted_i) {
+    float *p = (float *)malloc((size_t)V * 4);
+    NorProbIndex *pi = (NorProbIndex *)malloc((size_t)V * sizeof *pi), *tmp = (NorProbIndex *)malloc((size_t)V * sizeof *pi);
+    for (uint32_t q = 0; q < V; q++) p[q] = logits[q] / temperature;            /* infer.c:1174-1176 */
+    nor_softmax(p, (int)V);                                                     /* :1178 */
+    const float cutoff = (1.0f - top_p) / (float)((int)V - 1);                  /* :1064 */
+    uint32_t n0 = 0;
+    for (uint32_t i = 0; i < V; i++)
+        if (p[i] >= cutoff) { pi[n0].index = i; pi[n0].prob = p[i]; n0++; }
+    nor_sort_stable(pi, tmp, n0);
+    memset(out, 0, 9 * sizeof(uint32_t));
+    out[7] = n0;
+    for (uint32_t i = 0; i < 6; i++) out[1 + i] = n0 > i ? pi[i].index : 0u;
+    if (sorted_p) for (uint32_t i = 0; i < n0; i++) sorted_p[i] = pi[i].prob;
+    if (sorted_i) for (uint32_t i = 0; i < n0; i++) sorted_i[i] = pi[i].index;
+    if (n0 == 0) {
+        uint32_t best = 0;
+        for (uint32_t i = 1; i < V; i++) if (p[i] > p[best]) best = i;
+        out[0] = best; out[8] = 0xffffffffu;
+    } else {
+        float cum = 0.0f;                                                       /* :1075-1083 */
+        uint32_t last = n0 - 1;
+        for (uint32_t i = 0; i < n0; i++) { cum += pi[i].prob; if (cum > top_p) { last = i; break; } }
+        const float r = coin * cum;                                             /* :1099-1108 */
+        float cdf = 0.0f;
+        uint32_t pick = last;
+        for (uint32_t i = 0; i <= last; i++) { cdf += pi[i].prob; if (r < cdf) { pick = i; break; } }
+        out[0] = pi[pick].index; out[8] = last;
+    }
+    free(p); free(pi); free(tmp);
+}
+
+/* ------------------------------------------------------------------------------------------ */
 /* glibc-independent float exp used by the exact-mode CUDA path is validated against expf here */
 /* ------------------------------------------------------------------------------------------ */
 float nor_expf(float v) { return expf(v); }

@@ -8,7 +8,8 @@
  *     infer.c:756 ff., and calloc's the context, infer.c:553, so stock binaries crash);
  *   - lets a test copy FwdBuffer fields at a chosen (layer, phase) hook (infer.h:65-76 phases);
  *   - exposes the embedded sort model (main_sort.c:6) which is the reference's only golden fixture;
- *   - exposes llm_forward (infer.c:971, non-static but un-headered).
+ *   - exposes llm_forward (infer.c:971, non-static but un-headered);
+ *   - records the six ids of the last sampling observation (orh_last_sample).
  * Everything else (quantize, matmul_quant, matmul_q4k, rmsnorm, ...) is called straight through
  * ctypes on the reference's own non-static symbols.
  */
@@ -55,8 +56,14 @@ static float *orh_field(Nano_Context *ctx, int field) {
     }
 }
 
+static uint32_t g_last_sample[6];
+
 static void orh_hook(Nano_Observation obs, void *env) {
     Nano_Context *ctx = (Nano_Context *)env;
+    if (obs.layer == -1 && obs.phase == NANO_LLM_PHASE_SAMPLE) {      /* sample_top_p's six ids (infer.c:1086-1095) */
+        g_last_sample[0] = obs.token_0; g_last_sample[1] = obs.token_1; g_last_sample[2] = obs.token_2;
+        g_last_sample[3] = obs.token_3; g_last_sample[4] = obs.token_4; g_last_sample[5] = obs.token_5;
+    }
     for (int i = 0; i < g_nprobes; i++) {
         OrhProbe *p = &g_probes[i];
         if (p->layer == obs.layer && p->phase == obs.phase) {
@@ -121,6 +128,9 @@ int orh_probe_add(int32_t layer, int32_t phase, int32_t field, float *dst, uint3
     g_probes[g_nprobes] = (OrhProbe){layer, phase, field, dst, count, 0};
     return g_nprobes++;
 }
+
+/* token_0..5 of the last (layer -1, SAMPLE) observation */
+void orh_last_sample(uint32_t out[6]) { memcpy(out, g_last_sample, sizeof g_last_sample); }
 
 uint32_t orh_probe_hits(int idx) { return (idx >= 0 && idx < g_nprobes) ? g_probes[idx].hits : 0; }
 

@@ -90,9 +90,11 @@ def test_generate_next_token_greedy_matches_reference(penalty, monkeypatch):
 @needs_refhost
 @pytest.mark.skipif(not ob.ref_available("strict"), reason="needs the unmodified reference for the sampling path")
 @pytest.mark.parametrize("host_sampler", ["0", "1"], ids=["device-sampler", "host-sampler"])
-@pytest.mark.parametrize("name,quant,gs", [("toy-nano", mf.QUANT_Q80, 64), ("mini-qwen3", mf.QUANT_Q80, 128)])
+@pytest.mark.parametrize("name,quant,gs", [("toy-nano", mf.QUANT_Q80, 64), ("mini-qwen3", mf.QUANT_Q80, 128),
+                                           ("v16k-nano", mf.QUANT_Q80, 128), ("v152k-qwen3", mf.QUANT_Q80, 64)])
 def test_temperature_sampling_matches_reference(name, quant, gs, host_sampler, monkeypatch):
-    """temperature 0.7 / top-p 0.8 (main_cli.c:227) over 60 (toy-nano) / 96 (mini-qwen3) sampled steps: with bit-identical logits (exact mode) and the reference's own xorshift
+    """temperature 0.7 / top-p 0.8 (main_cli.c:227) over 60 (toy-nano) / 96 (the others) sampled steps, at V = 512, 4096, 16384 (Nano-168M)
+    and 151936 (Qwen3; the top-p scan stops many 4096-entry chunks in): with bit-identical logits (exact mode) and the reference's own xorshift
     coin, the ids equal the unmodified strict reference's -- for the device-side sampler (softmax, cutoff, stable descending order,
     sequential top-p scan on the GPU; 32 bytes back per token) and for the host restatement (NB200_HOST_SAMPLER=1, logits D2H)."""
     monkeypatch.setenv("NB200_EXACT", "1")
