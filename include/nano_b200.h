@@ -64,7 +64,12 @@ typedef struct nb200_config {
     uint32_t q_dim, kv_dim, max_seq_len;
     uint32_t tp_rank, tp_size;
     uint32_t reserved[7];   /* [0] execution path: 4 streaming kernel, 1 CUDA graph, 0 direct launches; [1], [2] creation-time calibration:
-                               us per token of the streaming kernel / of the multi-kernel graph (0 = the choice was not measured) */
+                               us per token of the streaming kernel / of the multi-kernel graph (0 = the choice was not measured);
+                               multi-kernel path, recorded when a kernel is launched or captured into the graph:
+                               [3] matvec variants used since creation, bit 3 * epilogue + {0: RB 1, 1: RB 2, 2: RB 4} with the
+                                   epilogues store 0, qkv 1, residual 2, swiglu 3, classifier 4 (the exact-mode F32 kernel sets none);
+                               [4] attention kernel of the last layer run: 0 none yet, 1 exact, 2 generic split-KV,
+                                   3 | kv_mul << 8 the split-KV kernel specialised for that kv_mul */
 } nb200_config;
 
 /* fields readable with nb200_read_buffer (same numbering as oracle probes) */

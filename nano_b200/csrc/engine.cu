@@ -111,6 +111,7 @@ struct nb200_engine {
     unsigned int *bar = nullptr;
     uint64_t launches = 0, weight_bytes = 0;
     uint32_t launches_per_token = 0;
+    uint32_t mv_mask = 0, attn_kind = 0;      // multi-kernel variants launched or captured so far (nb200_config.reserved[3], [4])
     std::vector<uint32_t> seen_mirror;   // ids whose seen[] flag is set, by position
     bool seen_valid = false;
     std::vector<void *> allocs;
@@ -155,7 +156,12 @@ int launch(nb200_engine *e, void (*kern)(const Args), dim3 grid, dim3 block, siz
         attr[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = attr; cfg.numAttrs = 1;
     }
-    if (smem > 48 * 1024) CK(cudaFuncSetAttribute((const void *)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // the 48 KB default covers static + dynamic shared memory together: a dynamic size just under 48 KB needs the opt-in too
+    if (smem > 40 * 1024) {
+        cudaFuncAttributes fa;
+        CK(cudaFuncGetAttributes(&fa, (const void *)kern));
+        if (smem + fa.sharedSizeBytes > 48 * 1024) CK(cudaFuncSetAttribute((const void *)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
     if (e && e->prof_on) {
         nb200_engine::ProfRec r{e->prof_tag, nullptr, nullptr};
         CK(cudaEventCreate(&r.a)); CK(cudaEventCreate(&r.b));
@@ -174,16 +180,18 @@ typedef void (*MatvecKern)(const MatvecArgs);
 
 template <int QUANT, int EPI, bool TP>
 MatvecKern pick_matvec(int rb, int lpg) {
-    if (QUANT == 0x80) {
+    // constexpr: F32 / Q4K must not instantiate the Q80 (RB, LPG) table (92 kernels no selection could reach)
+    if constexpr (QUANT == 0x80) {
 #define NB_PICK(RB_, L_) if (rb == RB_ && lpg == L_) return k_matvec<QUANT, EPI, RB_, L_, TP>;
         if constexpr (EPI != EPI_SWIGLU) { NB_PICK(1, 2) NB_PICK(1, 4) NB_PICK(1, 8) NB_PICK(1, 16) }      // SwiGLU pairs rows: RB even
         NB_PICK(2, 2) NB_PICK(2, 4) NB_PICK(2, 8) NB_PICK(2, 16)
         NB_PICK(4, 2) NB_PICK(4, 4) NB_PICK(4, 8) NB_PICK(4, 16)
 #undef NB_PICK
         return nullptr;
+    } else {
+        if (rb == 2) return k_matvec<QUANT, EPI, 2, 8, TP>;
+        return k_matvec<QUANT, EPI, 4, 8, TP>;
     }
-    if (rb == 2) return k_matvec<QUANT, EPI, 2, 8, TP>;
-    return k_matvec<QUANT, EPI, 4, 8, TP>;
 }
 
 template <int EPI>
@@ -232,6 +240,12 @@ int run_matvec(nb200_engine *e, int epi, const Mat &m, MatvecArgs a, bool norm, 
     int rb = (m.rows >= total_warps * 8) ? 4 : 2;
     // few long rows (O / W2 of the larger models): one row per warp keeps every warp busy, 4 tiles in flight each
     if (d.quant == 0x80u && epi != EPI_SWIGLU && m.rows <= total_warps && m.n >= 2048 && !getenv("NB200_NO_RB1")) rb = 1;
+    // NB200_MATVEC_RB=1|2|4 forces the row block (tests): RB = 1 exists for Q80 matrices other than W1|W3 only, the others keep 2
+    if (const char *f = getenv("NB200_MATVEC_RB")) {
+        const int want = atoi(f);
+        if (want == 2 || want == 4) rb = want;
+        else if (want == 1) rb = (d.quant == 0x80u && epi != EPI_SWIGLU) ? 1 : 2;
+    }
     const int lpg = (d.quant == 0x80u) ? (int)(d.gs / 16) : 8;
     MatvecKern k = nullptr;
     const bool tp = a.tp.size > 1;
@@ -248,6 +262,7 @@ int run_matvec(nb200_engine *e, int epi, const Mat &m, MatvecArgs a, bool norm, 
     const uint32_t cap = (uint32_t)num_sms * grid_mult();
     if (grid > cap) grid = cap;
     if (epi == EPI_CLS && e) { if (grid > e->cls_grid) grid = e->cls_grid; }
+    if (e) e->mv_mask |= 1u << (3 * epi + (rb == 1 ? 0 : rb == 2 ? 1 : 2));
     return launch<MatvecArgs>(e, k, dim3(grid), dim3(kThreads), smem, a);
 }
 
@@ -325,6 +340,7 @@ int run_layer(nb200_engine *e, uint32_t l) {
             }
             if (kern != k_attention) smem = attn_fast_smem_floats(d.kv_mul, d.hd, e->chunk_cap, e->nsplit_max, kWarps) * 4u;
         }
+        e->attn_kind = (kern == k_attention) ? 2u : (3u | (d.kv_mul << 8));
         if ((r = launch<AttnArgs>(e, kern, dim3(e->nsplit_max, d.KV), dim3(kern != k_attention ? kThreads : kAttnThreads), smem, a))) return r;
     } else {
         AttnExactArgs a{};
@@ -332,6 +348,7 @@ int run_layer(nb200_engine *e, uint32_t l) {
         a.qnorm = e->qnorm ? e->qnorm + (size_t)l * d.hd : nullptr;
         a.knorm = e->knorm ? e->knorm + (size_t)l * d.hd : nullptr;
         a.rope_cos = e->rope_cos; a.rope_sin = e->rope_sin; a.xba = e->xba; a.att = e->att_exact; a.st = e->st; a.d = d;
+        e->attn_kind = 1u;
         if ((r = launch<AttnExactArgs>(e, k_attention_exact, dim3(d.H), dim3(kAttnThreads), 2 * d.hd * 4, a))) return r;
     }
     if (e->lora.active) {   // o branch on the attention output; added to the O result before the residual (infer.c:898-903)
@@ -426,7 +443,7 @@ int capture_graph(nb200_engine *e) {
     cudaError_t ce = cudaStreamEndCapture(e->stream, &g);
     e->launches_per_token = (uint32_t)(e->launches - before);
     e->launches = before;
-    if (r) { if (g) cudaGraphDestroy(g); return r; }
+    if (r) { if (g) cudaGraphDestroy(g); cudaGetLastError(); return r; }     // the invalidated capture must not reach the next caller's error check
     if (ce != cudaSuccess) return fail(NB200_ECUDA, "graph capture failed: %s", cudaGetErrorString(ce));
     ce = cudaGraphInstantiate(&e->graph, g, 0);
     cudaGraphDestroy(g);
@@ -1134,6 +1151,8 @@ int nb200_get_config(const nb200_engine *e, nb200_config *c) {
     c->reserved[0] = e->use_stream ? 4u : (e->graph ? 1u : 0u);      // execution path: 4 streaming kernel, 1 graph, 0 direct launches
     c->reserved[1] = (uint32_t)(e->calib_ms[0] * 1000.0f + 0.5f);     // calibrate_paths: microseconds per token of the streaming kernel ...
     c->reserved[2] = (uint32_t)(e->calib_ms[1] * 1000.0f + 0.5f);     // ... and of the multi-kernel graph (0 = the choice was not measured)
+    c->reserved[3] = e->mv_mask;
+    c->reserved[4] = e->attn_kind;
     return 0;
 }
 
@@ -1404,7 +1423,7 @@ int op_prep(uint32_t quant, const float *x, const float *gain, uint32_t n, uint3
     CK(cudaMemcpy(dx.p, x, (size_t)n * 4, cudaMemcpyHostToDevice));
     if (gain) CK(cudaMemcpy(dg.p, gain, (size_t)n * 4, cudaMemcpyHostToDevice));
     const uint32_t smem = act_smem_bytes(quant, n, gs ? gs : 1);
-    if (smem > 48 * 1024) CK(cudaFuncSetAttribute((const void *)k_op_prep, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (smem > 40 * 1024) CK(cudaFuncSetAttribute((const void *)k_op_prep, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   // + static red[32]: see launch()
     k_op_prep<<<1, kThreads, smem>>>(dx.as<float>(), gain ? dg.as<float>() : nullptr, n, gs, quant, exact, dout.as<float>(),
                                      dcodes.as<int8_t>(), dscales.as<float>());
     CK(cudaGetLastError());

@@ -20,6 +20,7 @@ i8p = C.POINTER(C.c_int8)
 
 FLAG_EXACT, FLAG_NO_GRAPH, FLAG_NO_PDL, FLAG_NO_STREAM = 0x1, 0x2, 0x4, 0x10
 F_X, F_XBA, F_HB, F_Q, F_LOGITS, F_KROW, F_VROW, F_ACT_I8, F_ACT_SCALE = 0, 2, 4, 6, 9, 13, 14, 20, 21
+MATVEC_EPILOGUES = ("store", "qkv", "resid", "swiglu", "cls")      # kernels.cuh `Epilogue`, in value order
 
 EXPORTS = [
     "nb200_last_error", "nb200_device_count", "nb200_engine_create", "nb200_engine_destroy", "nb200_get_config",
@@ -142,6 +143,17 @@ class Engine:
         # creation-time calibration of the two fast paths (large one-GPU Q80 engines): us per token of each, None when not measured
         self.calibration = ({"streaming_us_per_token": int(cfg.reserved[1]), "multikernel_us_per_token": int(cfg.reserved[2])}
                             if int(cfg.reserved[1]) and int(cfg.reserved[2]) else None)
+
+    def kernels(self) -> dict:
+        """Kernels of the multi-kernel path this engine has launched or captured (include/nano_b200.h, reserved[3] / [4]):
+        {"matvec": set of (epilogue, RB), "attention": "exact" | "generic" | "fast<KVM>" | None}.  Read afresh on every call:
+        direct launches record a kernel on its first use, a captured graph at creation."""
+        cfg = Config()
+        _check(lib().nb200_get_config(self.h, C.byref(cfg)))
+        mask, att = int(cfg.reserved[3]), int(cfg.reserved[4])
+        mv = {(epi, rb) for i, epi in enumerate(MATVEC_EPILOGUES) for j, rb in enumerate((1, 2, 4)) if mask >> (3 * i + j) & 1}
+        kind = {0: None, 1: "exact", 2: "generic", 3: f"fast<{att >> 8}>"}[att & 0xff]
+        return {"matvec": mv, "attention": kind}
 
     # ---- LoRA plug-in ----
     def lora_load(self, image: bytes) -> None:

@@ -109,6 +109,20 @@ PRESETS: Dict[str, ModelSpec] = {
     "ffn7936-nano": ModelSpec("ffn7936-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 7936),      # Q4K: one block past it
     "ffn11520-nano": ModelSpec("ffn11520-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 11520),   # Q80 / F32: st_prep_max_n
     "ffn11648-nano": ModelSpec("ffn11648-nano", ARCH_NANO, 64, 512, 2, 256, 4, 2, 11648),   # Q80 / F32: one group past it
+    # 2-layer shapes of the multi-kernel path (tests/test_gpu_multikernel_matrix.py): the generic split-KV attention kernel
+    # (kv_mul outside {1, 2, 4, 8}, hd > 128, a Qwen3 hd that is not a power of two), k_attention_fast<8> where the merge's
+    # shared-memory cap cuts the split count, and the matvec row-block variants
+    "kvm3-qwen3": ModelSpec("kvm3-qwen3", ARCH_QWEN3, 2048, 1024, 2, 512, 6, 2, 1024, 128),
+    "kvm5-qwen3": ModelSpec("kvm5-qwen3", ARCH_QWEN3, 2048, 1024, 2, 512, 10, 2, 1024, 128),    # the Qwen3-14B ratio
+    "kvm7-nano": ModelSpec("kvm7-nano", ARCH_NANO, 2048, 1024, 2, 896, 14, 2, 2432),            # the Qwen2.5-0.5B layout
+    "mqa-qwen3": ModelSpec("mqa-qwen3", ARCH_QWEN3, 2048, 1024, 2, 512, 16, 1, 1024, 64),
+    "hd96-qwen3": ModelSpec("hd96-qwen3", ARCH_QWEN3, 2048, 1024, 2, 512, 8, 4, 1024, 96),
+    "hd192-nano": ModelSpec("hd192-nano", ARCH_NANO, 2048, 1024, 2, 768, 4, 2, 2048),
+    "hd512-qwen3": ModelSpec("hd512-qwen3", ARCH_QWEN3, 2048, 1024, 2, 512, 2, 1, 1024, 512),    # the engine's head_dim limit
+    "kvm8-qwen3": ModelSpec("kvm8-qwen3", ARCH_QWEN3, 2048, 1024, 2, 512, 16, 2, 1024, 128),
+    # V = 4099 = 3 (mod 4): the classifier's last row block is partial at RB 2 and 4; F = 5376 = 21 * 256 takes every group
+    # size, and W2's K loop runs past one group of four 1024-byte tiles into a partial tile
+    "mv-nano": ModelSpec("mv-nano", ARCH_NANO, 2048, 4099, 2, 512, 4, 2, 5376),
     # 2-layer models with the real vocabularies (Nano-168M, Qwen3): the sampler's scans over many 4096-entry chunks
     # (tests/test_gpu_sampler.py, tests/test_gpu_shim.py)
     "v16k-nano": ModelSpec("v16k-nano", ARCH_NANO, 128, 16384, 2, 256, 4, 2, 512),

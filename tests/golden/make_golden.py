@@ -17,7 +17,7 @@ Run in the build container (needs /root/reference):   python tests/golden/make_g
                        of its F32 / Q80 / LoRA files, the model's RoPE tables and its PyTorch logits over 12 teacher-forced
                        positions:  python tests/golden/make_golden.py --export
   reference_noise_floor.json  max |fast build - strict build| of the reference's logits per quantised test file; the floors of
-                       the stream-matrix files alone:  python tests/golden/make_golden.py --floors
+                       the stream- and multi-kernel-matrix files alone:  python tests/golden/make_golden.py --floors
 """
 import ctypes as C
 import hashlib
@@ -55,8 +55,22 @@ def sha(a) -> str:
     return hashlib.sha256(a if isinstance(a, bytes) else np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
+def file_variants(name, group_sizes=(32, 128, 256)):
+    """(quant, gs) of every file kind a preset's shape allows: F32, Q80 with each group size dividing n_embd, q_dim and
+    n_hidden, Q4K when 256 divides them."""
+    spec = mf.PRESETS[name]
+    dims = (spec.n_embd, spec.q_dim, spec.n_hidden)
+    out = [(mf.QUANT_F32, 128)] + [(mf.QUANT_Q80, g) for g in group_sizes if all(n % g == 0 for n in dims)]
+    return out + ([(mf.QUANT_Q4K, 128)] if all(n % 256 == 0 for n in dims) else [])
+
+
+# the files of tests/test_gpu_multikernel_matrix.py: the attention presets, and the matvec preset with every group size
+MULTI_ATTN_PRESETS = ["kvm3-qwen3", "kvm5-qwen3", "kvm7-nano", "mqa-qwen3", "hd96-qwen3", "hd192-nano", "hd512-qwen3", "kvm8-qwen3"]
+MULTI_CASES = ([(n, q, g) for n in MULTI_ATTN_PRESETS for q, g in file_variants(n)] +
+               [("mv-nano", q, g) for q, g in file_variants("mv-nano", (32, 64, 128, 256))])
+
 # shared with the tests that compare against these digests
-STRICT_CASES = TOY_CONFIGS + [("toy-nano-odd", mf.QUANT_F32, 128), ("mini-qwen3", mf.QUANT_Q80, 128)]
+STRICT_CASES = TOY_CONFIGS + [("toy-nano-odd", mf.QUANT_F32, 128), ("mini-qwen3", mf.QUANT_Q80, 128)] + MULTI_CASES
 STRICT_SEQ = 20
 LORA_CASES = [(mf.QUANT_F32, 128), (mf.QUANT_Q80, 64), (mf.QUANT_Q4K, 128)]
 LORA_KV_POSITIONS = [0, 5, TOY_SEQ - 1]
@@ -153,7 +167,8 @@ MATRIX_FLOOR_CASES = ([(n, q, g) for n in ("kvm1-nano", "kvm4-qwen3-hd128", "kvm
                       [("qwen3-4b-2l", mf.QUANT_Q80, 128), ("ffn3968-nano", mf.QUANT_Q80, 128), ("ffn3968-nano", mf.QUANT_Q80, 64),
                        ("ffn4096-nano", mf.QUANT_Q4K, 128), ("ffn4096-nano", mf.QUANT_Q80, 64), ("ffn7680-nano", mf.QUANT_Q4K, 128),
                        ("ffn7680-nano", mf.QUANT_Q80, 128), ("ffn11520-nano", mf.QUANT_Q80, 128), ("ffn11520-nano", mf.QUANT_Q80, 64),
-                       ("ffn7936-nano", mf.QUANT_Q4K, 128), ("ffn7936-nano", mf.QUANT_Q80, 128), ("ffn11648-nano", mf.QUANT_Q80, 128)])
+                       ("ffn7936-nano", mf.QUANT_Q4K, 128), ("ffn7936-nano", mf.QUANT_Q80, 128), ("ffn11648-nano", mf.QUANT_Q80, 128)] +
+                      [c for c in MULTI_CASES if c[1] != mf.QUANT_F32])
 
 
 def noise_floors(cases, S=40):
@@ -300,7 +315,7 @@ if __name__ == "__main__":
         reference_digests()
     elif "--export" in sys.argv:
         export_digests()
-    elif "--floors" in sys.argv:           # add the stream-matrix floors to the committed ones
+    elif "--floors" in sys.argv:           # add the floors of the stream- and multi-kernel-matrix files to the committed ones
         ob.build()
         path = os.path.join(HERE, "reference_noise_floor.json")
         floors = json.load(open(path))
