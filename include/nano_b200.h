@@ -123,6 +123,10 @@ int nb200_lora_unload(nb200_engine *e);
 
 int nb200_get_config(const nb200_engine *e, nb200_config *cfg);
 
+/* Positions: every call that takes one refuses pos >= min(max_seq_len, block_size) with NB200_EINVAL.  The RoPE table has
+ * block_size rows, so a position past it has no defined result (the reference reads past its table there).  A context with
+ * max_seq_len > block_size is still legal; its rows from block_size on stay zero and non-causal attention reads them as such. */
+
 /* one token through the network; logits stay in HBM.  is_causal=0 is the reference's seq2seq mode
  * (attention over all max_seq_len cache rows, infer.c:849). */
 int nb200_forward(nb200_engine *e, uint32_t token, uint32_t pos, uint32_t is_causal);
@@ -145,7 +149,7 @@ int nb200_next_sampled(nb200_engine *e, const uint32_t *ids, uint32_t pos, float
 /* Device-resident greedy loop: ids[0..n_prompt) is the prompt; positions 0..n_total-2 are run and
  * ids[n_prompt..n_total) are filled with greedy tokens (prompt positions are teacher-forced exactly like
  * llm_session_step).  device_ms (optional) receives the CUDA-event time of the decode segment
- * (positions >= n_prompt-1); prefill_ms the prompt segment. */
+ * (positions >= n_prompt-1); prefill_ms the prompt segment.  n_total <= min(max_seq_len, block_size) + 1. */
 int nb200_decode_greedy(nb200_engine *e, uint32_t *ids, uint32_t n_prompt, uint32_t n_total,
                         float repetition_penalty, float *prefill_ms, float *device_ms);
 

@@ -685,6 +685,10 @@ static int calibrate_paths(nb200_engine *e);
 static int push_state(nb200_engine *e, uint32_t pos, uint32_t causal, uint32_t n_prompt, uint32_t advance, float penalty,
                       uint32_t token, uint32_t use_token);
 
+// Positions [0, pos_limit) are the ones a call may run: the device RoPE table holds min(block_size, max_seq) rows, and the
+// kernels index it by position unguarded.  Rows from block_size to max_seq of a longer context stay zero.
+static uint32_t pos_limit(const Dims &d) { return d.block_size < d.max_seq ? d.block_size : d.max_seq; }
+
 static int create_impl(nb200_engine **out, const uint8_t *img, uint64_t image_bytes, uint32_t max_seq_len, int device,
                        uint32_t flags, uint32_t tp_rank, uint32_t tp_size) {
     if (!out || !img || image_bytes < 260 || max_seq_len == 0) return fail(NB200_EINVAL, "bad arguments");
@@ -810,7 +814,7 @@ static int create_impl(nb200_engine **out, const uint8_t *img, uint64_t image_by
     }
     {   // RoPE tables: rows [0, min(block_size, max_seq)) are the only ones a context of max_seq can index
         const uint32_t half = d.hd / 2;
-        const uint32_t nrows = d.block_size < d.max_seq ? d.block_size : d.max_seq;
+        const uint32_t nrows = pos_limit(d);
         const size_t tb = (size_t)nrows * half * 4;
         DM(e->rope_cos, tb); DM(e->rope_sin, tb);
         if (d.arch == 3u) {   // rebuilt with theta = 1e6 on the host libm, exactly infer.c:189-204
@@ -976,13 +980,15 @@ static int finish_paths(nb200_engine *e) {
     return 0;
 }
 
-// Both fast paths are ready: time `n` decode steps on each from the middle of the context (device loop, CUDA events on the engine's
-// stream, one untimed round first) and keep the faster.  The steps write K/V rows at positions pos0.. -- every later step rewrites its
-// own position before reading it -- and leave no other state behind (push_state precedes every public entry point).
+// Both fast paths are ready: time `n` decode steps on each from the middle of the usable context (device loop, CUDA events on the
+// engine's stream, one untimed round first) and keep the faster.  The steps write K/V rows at positions pos0.., logits, x and the
+// ids; all of it is cleared again afterwards, because non-causal attention reads every cache row, written or not, and a fresh
+// engine must compute what the reference's calloc'd context does.
 static int calibrate_paths(nb200_engine *e) {
     const uint32_t n = 8;
-    if (e->d.max_seq < 4 * n) return 0;
-    const uint32_t pos0 = e->d.max_seq / 2;
+    const uint32_t lim = pos_limit(e->d);
+    if (lim < 4 * n) return 0;
+    const uint32_t pos0 = lim / 2;
     struct Events { cudaEvent_t ev[2] = {nullptr, nullptr}; ~Events() { for (auto v : ev) if (v) cudaEventDestroy(v); } } evs;
     for (auto &v : evs.ev) CK(cudaEventCreate(&v));
     float ms[2] = {0.0f, 0.0f};
@@ -1006,8 +1012,12 @@ static int calibrate_paths(nb200_engine *e) {
     e->path_stream = e->use_stream;
     if (e->use_stream) e->launches_per_token = 1;
     e->launches = 0;
-    CK(cudaMemsetAsync(e->ids_dev, 0, ((size_t)e->d.max_seq + 8) * 4, e->stream));       // as created
-    CK(cudaMemsetAsync(e->seen, 0, e->d.V, e->stream));
+    const Dims &d = e->d;                                                                 // as created
+    const size_t kv_floats = (size_t)d.L * d.KV * d.max_seq * d.hd;
+    CK(cudaMemsetAsync(e->kc, 0, kv_floats * 4, e->stream)); CK(cudaMemsetAsync(e->vc, 0, kv_floats * 4, e->stream));
+    CK(cudaMemsetAsync(e->x, 0, (size_t)d.E * 4, e->stream)); CK(cudaMemsetAsync(e->logits, 0, (size_t)d.V * 4, e->stream));
+    CK(cudaMemsetAsync(e->ids_dev, 0, ((size_t)d.max_seq + 8) * 4, e->stream));
+    CK(cudaMemsetAsync(e->seen, 0, d.V, e->stream));
     e->seen_valid = false; e->seen_mirror.clear();
     CK(cudaStreamSynchronize(e->stream));
     return 0;
@@ -1178,7 +1188,7 @@ static int push_state(nb200_engine *e, uint32_t pos, uint32_t causal, uint32_t n
 
 int nb200_forward(nb200_engine *e, uint32_t token, uint32_t pos, uint32_t is_causal) {
     if (!e) return fail(NB200_EINVAL, "null engine");
-    if (pos >= e->d.max_seq || token >= e->d.V) return fail(NB200_EINVAL, "token/pos out of range");
+    if (pos >= pos_limit(e->d) || token >= e->d.V) return fail(NB200_EINVAL, "token/pos out of range");
     CK(cudaSetDevice(e->device));
     int r;
     if ((r = push_state(e, pos, is_causal ? 1u : 0u, 0, 0, 1.0f, token, 1))) return r;
@@ -1215,7 +1225,7 @@ static int sync_seen(nb200_engine *e, const uint32_t *ids, uint32_t pos) {
 
 int nb200_next_greedy(nb200_engine *e, const uint32_t *ids, uint32_t pos, int is_prefilling, float penalty, uint32_t *next) {
     if (!e || !ids || !next) return fail(NB200_EINVAL, "null argument");
-    if (pos >= e->d.max_seq || ids[pos] >= e->d.V) return fail(NB200_EINVAL, "token/pos out of range");
+    if (pos >= pos_limit(e->d) || ids[pos] >= e->d.V) return fail(NB200_EINVAL, "token/pos out of range");
     CK(cudaSetDevice(e->device));
     int r;
     if ((r = push_state(e, pos, 1, 0, 0, is_prefilling ? 1.0f : penalty, ids[pos], 1))) return r;
@@ -1232,7 +1242,7 @@ int nb200_next_greedy(nb200_engine *e, const uint32_t *ids, uint32_t pos, int is
 int nb200_next_sampled(nb200_engine *e, const uint32_t *ids, uint32_t pos, float penalty, float temperature, float top_p, float coin,
                        uint32_t *next, uint32_t *top6) {
     if (!e || !ids || !next) return fail(NB200_EINVAL, "null argument");
-    if (pos >= e->d.max_seq || ids[pos] >= e->d.V) return fail(NB200_EINVAL, "token/pos out of range");
+    if (pos >= pos_limit(e->d) || ids[pos] >= e->d.V) return fail(NB200_EINVAL, "token/pos out of range");
     if (!(temperature > 0.0f)) return fail(NB200_EINVAL, "temperature must be > 0 (use nb200_next_greedy for 0)");
     if (e->tp_size > 1) return fail(NB200_EINVAL, "device-side sampling is not available on tensor-parallel engines (logits are sharded)");
     CK(cudaSetDevice(e->device));
@@ -1258,7 +1268,7 @@ int nb200_next_sampled(nb200_engine *e, const uint32_t *ids, uint32_t pos, float
 int nb200_decode_greedy(nb200_engine *e, uint32_t *ids, uint32_t n_prompt, uint32_t n_total, float penalty,
                         float *prefill_ms, float *device_ms) {
     if (!e || !ids) return fail(NB200_EINVAL, "null argument");
-    if (n_prompt < 1 || n_total < n_prompt || n_total > e->d.max_seq + 1) return fail(NB200_EINVAL, "bad n_prompt/n_total");
+    if (n_prompt < 1 || n_total < n_prompt || n_total > pos_limit(e->d) + 1) return fail(NB200_EINVAL, "bad n_prompt/n_total");
     for (uint32_t i = 0; i < n_prompt; i++) if (ids[i] >= e->d.V) return fail(NB200_EINVAL, "id out of range");
     CK(cudaSetDevice(e->device));
     int r;
@@ -1329,7 +1339,7 @@ int nb200_write_x(nb200_engine *e, const float *x, uint32_t count) {
 }
 
 int nb200_run_layer(nb200_engine *e, uint32_t layer, uint32_t pos, uint32_t is_causal) {
-    if (!e || layer >= e->d.L || pos >= e->d.max_seq) return fail(NB200_EINVAL, "bad argument");
+    if (!e || layer >= e->d.L || pos >= pos_limit(e->d)) return fail(NB200_EINVAL, "bad argument");
     if (e->tp_size > 1) return fail(NB200_EINVAL, "not available on tensor-parallel engines");
     CK(cudaSetDevice(e->device));
     int r;
@@ -1344,7 +1354,7 @@ int nb200_run_layer(nb200_engine *e, uint32_t layer, uint32_t pos, uint32_t is_c
 // 0 embed, 1 qkv, 2 attention, 3 o-proj, 4 w1|w3, 5 w2, 6 classifier.
 int nb200_profile_tokens(nb200_engine *e, const uint32_t *ids, uint32_t start, uint32_t n, float ms[7], uint32_t counts[7]) {
     if (!e || !ids || !ms || !counts) return fail(NB200_EINVAL, "null argument");
-    if (start + n > e->d.max_seq) return fail(NB200_EINVAL, "range exceeds max_seq_len");
+    if (n > pos_limit(e->d) || start > pos_limit(e->d) - n) return fail(NB200_EINVAL, "range exceeds min(max_seq_len, block_size)");
     CK(cudaSetDevice(e->device));
     const bool pdl = e->use_pdl;
     e->use_pdl = false; e->prof_on = true;
@@ -1378,6 +1388,7 @@ int nb200_read_attn_trace(nb200_engine *e, unsigned long long *stamps32) {
 int nb200_trace_token(nb200_engine *e, uint32_t token, uint32_t pos, unsigned long long *stamps, uint32_t cap, uint32_t *count) {
     if (!e || !stamps || !count) return fail(NB200_EINVAL, "null argument");
     if (!e->use_stream) return fail(NB200_EINVAL, "persistent kernel not active");
+    if (pos >= pos_limit(e->d) || token >= e->d.V) return fail(NB200_EINVAL, "token/pos out of range");
     CK(cudaSetDevice(e->device));
     const uint32_t n = 1024 + 256;         // [0, 5L+2): per-barrier stamps; [1024, 1024+15): phase stamps of layer L/2; [1100, 1100+64): stamps inside its four matvec phases
     if (cap < n || 5 * e->d.L + 4 > 1024) return fail(NB200_EINVAL, "need room for %u stamps", n);

@@ -362,7 +362,8 @@ static wchar_t *detok(Nano_Context *ctx, uint32_t *ids, uint32_t n) {
 }
 
 int32_t llm_session_step(Nano_Context *ctx, Nano_Session *s) {
-    if (s->pos >= s->max_seq_len) return NANO_STOP_ERROR;
+    /* past the model's RoPE table no position has a defined result (the engine refuses it): end the session like at max_seq_len */
+    if (s->pos >= s->max_seq_len || s->pos >= ctx->llm->config.block_size) return NANO_STOP_ERROR;
     const uint32_t arch = ctx->llm->arch;
     if (arch != NANO_ARCH_NANO && arch != NANO_ARCH_QWEN2 && arch != NANO_ARCH_QWEN3) { printf("Error: unknown LLM arch.\n"); return NANO_STOP_ERROR; }
     if (s->output_text) { free(s->output_text); s->output_text = NULL; }

@@ -128,6 +128,9 @@ PRESETS: Dict[str, ModelSpec] = {
     "v16k-nano": ModelSpec("v16k-nano", ARCH_NANO, 128, 16384, 2, 256, 4, 2, 512),
     "v152k-qwen3": ModelSpec("v152k-qwen3", ARCH_QWEN3, 128, 151936, 2, 256, 4, 2, 512, 64),
     "v152k-qwen3-untied": ModelSpec("v152k-qwen3-untied", ARCH_QWEN3, 128, 151936, 2, 256, 4, 2, 512, 64, 0),
+    # 2 layers of the Qwen3-4B layer shape, V = 32768: ~295 MB of Q80 g128 weights, above the 256 MiB from which a one-GPU
+    # engine times both fast paths at creation (calibrate_paths; tests/test_gpu_sessions.py, written with fast=True)
+    "calib-qwen3": ModelSpec("calib-qwen3", ARCH_QWEN3, 256, 32768, 2, 2560, 32, 8, 9728, 128),
 }
 
 

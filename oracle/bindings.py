@@ -266,8 +266,19 @@ class RefEngine:
         self._lora_image = np.frombuffer(bytes(image), dtype=np.uint8).copy()
         self.L.orh_load_lora(self.h, self._lora_image.ctypes.data)
 
-    def forward(self, token: int, pos: int, causal: int = 1) -> np.ndarray:
-        p = self.L.orh_forward(self.h, int(token), int(pos), causal)
+    def forward(self, token: int, pos: int, causal: int = 1, lora: bool = True) -> np.ndarray:
+        """llm_forward with the loaded plug-in (lora=True, what generate_next_token passes) or without it (lora=False,
+        what seq2seq passes).  lora=False needs orh_forward_lora (see ref_has_forward_lora), bound here so that an older
+        harness serves lora=True."""
+        if lora:
+            p = self.L.orh_forward(self.h, int(token), int(pos), causal)
+        else:
+            if not hasattr(self.L, "orh_forward_lora"):
+                raise RuntimeError("the harness in oracle/_ref predates orh_forward_lora; rebuild it (oracle.bindings.build)")
+            f = self.L.orh_forward_lora
+            f.restype = f32p
+            f.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int]
+            p = f(self.h, int(token), int(pos), causal, 0)
         return np.ctypeslib.as_array(p, shape=(self.vocab,)).copy()
 
     def next(self, ids: np.ndarray, pos: int, prefilling: int) -> int:
@@ -309,6 +320,12 @@ def ref_last_sample(flavour: str = "strict"):
     f.argtypes = [u32p]
     f.restype = None
     return f
+
+
+def ref_has_forward_lora(flavour: str = "strict") -> bool:
+    """Whether the harness in oracle/_ref has orh_forward_lora (RefEngine.forward(..., lora=False)).  A harness built
+    before it existed still serves every other test; the tests that switch the plug-in per call skip, saying why."""
+    return ref_available(flavour) and hasattr(RefEngine.lib(flavour), "orh_forward_lora")
 
 
 def sort_model_bytes(flavour: str = "strict") -> bytes:

@@ -8,7 +8,7 @@
  *     infer.c:756 ff., and calloc's the context, infer.c:553, so stock binaries crash);
  *   - lets a test copy FwdBuffer fields at a chosen (layer, phase) hook (infer.h:65-76 phases);
  *   - exposes the embedded sort model (main_sort.c:6) which is the reference's only golden fixture;
- *   - exposes llm_forward (infer.c:971, non-static but un-headered);
+ *   - exposes llm_forward (infer.c:971, non-static but un-headered), with or without the loaded LoRA plug-in;
  *   - records the six ids of the last sampling observation (orh_last_sample).
  * Everything else (quantize, matmul_quant, matmul_q4k, rmsnorm, ...) is called straight through
  * ctypes on the reference's own non-static symbols.
@@ -105,6 +105,11 @@ void orh_load_lora(Nano_Context *ctx, uint8_t *buffer) {
 
 float *orh_forward(Nano_Context *ctx, uint32_t token, uint32_t pos, uint32_t is_causal) {
     return llm_forward(ctx, token, pos, ctx->max_seq_len, is_causal, ctx->llm, ctx->lora);
+}
+
+/* the plug-in per call, as the reference's own callers pass it (seq2seq passes NULL while ctx->lora is set, infer.c:1365-1402) */
+float *orh_forward_lora(Nano_Context *ctx, uint32_t token, uint32_t pos, uint32_t is_causal, int use_lora) {
+    return llm_forward(ctx, token, pos, ctx->max_seq_len, is_causal, ctx->llm, use_lora ? ctx->lora : NULL);
 }
 
 uint32_t orh_next(Nano_Context *ctx, uint32_t *ids, uint32_t pos, int is_prefilling) {

@@ -2,8 +2,9 @@
 
 The C oracle and the CUDA engine both compute in fp32; this computes the same function in float64 from the file's fp32
 parameters, so |engine - ref64| can be compared with |oracle - ref64|: the CUDA result must be as close to the exact
-answer as the reference-order fp32 computation is, within a small factor.  All teacher-forced positions are computed at
-once (a prefill with a causal mask), which is what the token-by-token decode computes position by position.
+answer as the reference-order fp32 computation is, within a small factor.  `forward` computes all teacher-forced positions
+at once (a prefill with a causal mask), which is what the token-by-token decode computes position by position.  `Session64`
+keeps the caches across calls as the engine does: rewinds, new sessions over stale rows and non-causal sweeps.
 
 Restated from the reference's forward pass (infer.c:713-1018): embedding, rmsnorm (eps 1e-5), Qwen3 per-head q/k rmsnorm,
 RoPE on adjacent pairs (Nano, tables read from the file) or on half-split pairs (Qwen3, table built from theta 1e6),
@@ -81,16 +82,26 @@ def _rope(h, cos, sin, halfsplit):
     return out
 
 
-def forward(spec, p, tokens):
-    """Teacher-forced prefill of `tokens`: (logits [S, V], k rows [L, S, kv_dim] post-RoPE, v rows [L, S, kv_dim])."""
+def _attend(q, k, v, mask):
+    """q [S, H, hd] against cache rows k / v [n, KV, hd] with an additive mask [S, n]: o [S, H, hd]"""
+    H, hd = q.shape[1], q.shape[2]
+    kvm = H // k.shape[1]
+    o = np.empty_like(q)
+    for h in range(H):
+        sc = (q[:, h, :] @ k[:, h // kvm, :].T) / np.sqrt(hd) + mask
+        sc = np.exp(sc - sc.max(axis=1, keepdims=True))
+        o[:, h, :] = (sc / sc.sum(axis=1, keepdims=True)) @ v[:, h // kvm, :]
+    return o
+
+
+def _layers(spec, p, tokens, positions, attention):
+    """The transformer blocks and the classifier for `tokens` at `positions`.  attention(l, q, k, v) receives this call's
+    post-RoPE q [S, H, hd], k / v [S, KV, hd] of layer l and returns the attention output [S, H, hd]."""
     S = len(tokens)
     H, KV, hd = spec.n_head, spec.n_kv_head, spec.hd
-    kvm = H // KV
     qwen3 = spec.arch == mf.ARCH_QWEN3
-    cos, sin = p["cos"][:S], p["sin"][:S]
-    mask = np.triu(np.full((S, S), -np.inf), 1)
+    cos, sin = p["cos"][positions], p["sin"][positions]
     x = p["emb"][np.asarray(tokens, dtype=np.int64)]
-    ks, vs = [], []
     for l in range(spec.n_layer):
         xb = _rmsnorm(x, p["attn_norm"][l])
         q = (xb @ p["wq"][l].T).reshape(S, H, hd)
@@ -99,15 +110,42 @@ def forward(spec, p, tokens):
         if qwen3:
             q, k = _rmsnorm(q, p["q_norm"][l]), _rmsnorm(k, p["k_norm"][l])
         q, k = _rope(q, cos, sin, qwen3), _rope(k, cos, sin, qwen3)
-        ks.append(k.reshape(S, KV * hd)); vs.append(v.reshape(S, KV * hd))
-        o = np.empty((S, H, hd))
-        for h in range(H):
-            sc = (q[:, h, :] @ k[:, h // kvm, :].T) / np.sqrt(hd) + mask
-            sc = np.exp(sc - sc.max(axis=1, keepdims=True))
-            o[:, h, :] = (sc / sc.sum(axis=1, keepdims=True)) @ v[:, h // kvm, :]
+        o = attention(l, q, k, v)
         x = x + o.reshape(S, H * hd) @ p["wo"][l].T
         xb = _rmsnorm(x, p["ffn_norm"][l])
         h1, h3 = xb @ p["w1"][l].T, xb @ p["w3"][l].T
         x = x + (h1 / (1.0 + np.exp(-h1)) * h3) @ p["w2"][l].T
-    logits = _rmsnorm(x, p["final_norm"]) @ p["emb"].T
+    return _rmsnorm(x, p["final_norm"]) @ p["emb"].T
+
+
+def forward(spec, p, tokens):
+    """Teacher-forced prefill of `tokens`: (logits [S, V], k rows [L, S, kv_dim] post-RoPE, v rows [L, S, kv_dim])."""
+    S = len(tokens)
+    mask = np.triu(np.full((S, S), -np.inf), 1)
+    ks, vs = [], []
+
+    def causal(l, q, k, v):
+        ks.append(k.reshape(S, -1)); vs.append(v.reshape(S, -1))
+        return _attend(q, k, v, mask)
+    logits = _layers(spec, p, tokens, np.arange(S), causal)
     return logits, np.stack(ks), np.stack(vs)
+
+
+class Session64:
+    """The engine's per-call state in float64: K / V caches [L][max_seq][kv_dim], zero at creation like the reference's
+    calloc'd context (infer.c:47).  forward(token, pos, causal) writes row pos of every layer before it attends, then
+    attends over rows [0, pos] (causal) or over all max_seq rows, written or not (seq2seq, infer.c:849)."""
+
+    def __init__(self, spec, p, max_seq):
+        self.spec, self.p, self.max_seq = spec, p, max_seq
+        self.k = np.zeros((spec.n_layer, max_seq, spec.kv_dim))
+        self.v = np.zeros((spec.n_layer, max_seq, spec.kv_dim))
+
+    def forward(self, token, pos, causal=1):
+        n = pos + 1 if causal else self.max_seq
+        KV, hd = self.spec.n_kv_head, self.spec.hd
+
+        def cached(l, q, k, v):
+            self.k[l, pos], self.v[l, pos] = k.reshape(-1), v.reshape(-1)
+            return _attend(q, self.k[l, :n].reshape(n, KV, hd), self.v[l, :n].reshape(n, KV, hd), np.zeros((1, n)))
+        return _layers(self.spec, self.p, [token], np.array([pos]), cached)[0]

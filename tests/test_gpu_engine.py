@@ -246,6 +246,13 @@ def test_rejects_bad_inputs():
         eng.forward(spec.vocab, 0)          # token out of range
     with pytest.raises(E.NB200Error):
         eng.forward(1, 8)                   # pos >= max_seq_len
+    ids = np.ones(10, np.uint32)
+    with pytest.raises(E.NB200Error):
+        eng.next_greedy(ids, 8, 0, 1.3)
+    with pytest.raises(E.NB200Error):
+        eng.next_sampled(ids, 8, 1.3, 0.7, 0.8, 0.5)
+    with pytest.raises(E.NB200Error):
+        eng.decode_greedy(ids, 2, 10)       # n_total > max_seq_len + 1
     eng.close()
     with pytest.raises(E.NB200Error):
         E.Engine(b"\0" * 4096, 8)           # bad magic

@@ -179,6 +179,27 @@ def test_ref64_matches_oracle_on_cpu():
             assert np.abs(ov[l, :S] - v[l]).max() <= 1e-5 * np.abs(v[l]).max(), (name, l, "V")
 
 
+def test_session64_matches_oracle_on_cpu():
+    """The float64 session (ref64.Session64) against the C oracle driven through the same calls: a teacher-forced run, a
+    rewind, a non-causal sweep over all rows (some never written) and a second session over stale rows.  fp32 noise only."""
+    for name in ("toy-nano", "toy-qwen3"):
+        spec = mf.PRESETS[name]
+        path = mf.cached_model(spec, F32, 128)
+        S = 32
+        o = ob.NanoOracle(path, S); s = ref64.Session64(*ref64.load_f32(path), S)
+        a, b = mf.teacher_tokens(S, spec.vocab), mf.teacher_tokens(S, spec.vocab, seed=7)
+        script = ([(a[p], p, 1) for p in range(24)] + [(b[p], p, 1) for p in range(8, 20)] +
+                  [(a[p], p, 0) for p in range(S)] + [(b[p], p, 1) for p in range(6)])
+        for tok, pos, causal in script:
+            lg32, lg64 = o.forward(tok, pos, causal), s.forward(tok, pos, causal)
+            assert np.abs(lg32 - lg64).max() <= 1e-5 * np.abs(lg64).max(), (name, pos, causal)
+        ok, ov = o.kv()
+        for l in range(spec.n_layer):
+            assert np.abs(ok[l] - s.k[l]).max() <= 1e-5 * np.abs(s.k[l]).max(), (name, l, "K")
+            assert np.abs(ov[l] - s.v[l]).max() <= 1e-5 * np.abs(s.v[l]).max(), (name, l, "V")
+        o.close()
+
+
 TIGHT_SHAPES = ["kvm1-nano", "long-qwen3", "hd52-nano", "kvm4-qwen3-hd128", "kvm4-qwen3-hd64"]     # KVM 1, 2, 2, 4, 4
 S_LONG = 2048
 # NB200_STAGE_KB=1: setup_stream raises the stage to the smallest one that holds a row unit of the widest matrix, so this is the

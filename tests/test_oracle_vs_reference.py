@@ -158,3 +158,22 @@ def test_lora_golden_is_what_the_reference_computes():
         for i, pos in enumerate(TOY_POSITIONS):
             assert sha(gold[key][i]) == REF_OUT["lora"][key]["logits"][pos], f"lora golden {quant:#x} pos {pos}"
             assert np.abs(gold[key][i] - base[key][i]).max() > 1e-2, "the plug-in must change the logits"
+
+
+@pytest.mark.skipif(not ob.ref_available("strict"), reason="needs the unmodified reference (oracle/_ref)")
+@pytest.mark.parametrize("quant,gs", LORA_CASES)
+def test_reference_harness_takes_the_plug_in_per_call(quant, gs):
+    """RefEngine.forward(..., lora=): with the plug-in loaded, lora=True is what the reference computes with it and lora=False
+    (what seq2seq passes) what it computes for the plain model -- both against the committed strict-reference digests."""
+    if not ob.ref_has_forward_lora():
+        pytest.skip("the reference harness in oracle/_ref predates orh_forward_lora (llm_forward without the plug-in)")
+    spec = mf.PRESETS["toy-nano"]
+    key = f"toy-nano_{quant:02x}_{gs}"
+    path = mf.cached_model(spec, quant, gs)
+    toks = mf.teacher_tokens(len(REF_OUT["lora"][key]["logits"]), spec.vocab)
+    r = ob.RefEngine(path, len(toks), "strict"); r.load_lora(mf.write_lora(spec, 8, 16, seed=7))
+    for pos, want in enumerate(REF_OUT["lora"][key]["logits"]):
+        assert sha(r.forward(toks[pos], pos, lora=True)) == want, f"with the plug-in, pos {pos}"
+    for pos, want in enumerate(REF_OUT["strict"][key]["logits"]):
+        assert sha(r.forward(toks[pos], pos, lora=False)) == want, f"without the plug-in, pos {pos}"
+    r.close()
