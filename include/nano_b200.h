@@ -69,7 +69,9 @@ typedef struct nb200_config {
                                [3] matvec variants used since creation, bit 3 * epilogue + {0: RB 1, 1: RB 2, 2: RB 4} with the
                                    epilogues store 0, qkv 1, residual 2, swiglu 3, classifier 4 (the exact-mode F32 kernel sets none);
                                [4] attention kernel of the last layer run: 0 none yet, 1 exact, 2 generic split-KV,
-                                   3 | kv_mul << 8 the split-KV kernel specialised for that kv_mul */
+                                   3 | kv_mul << 8 the split-KV kernel specialised for that kv_mul;
+                               nb200_prefill: [5] positions per chunk M (0 until the first call), [6] the attention kernel of the
+                                   last prefill, encoded as [4] */
 } nb200_config;
 
 /* fields readable with nb200_read_buffer (same numbering as oracle probes) */
@@ -152,6 +154,20 @@ int nb200_next_sampled(nb200_engine *e, const uint32_t *ids, uint32_t pos, float
  * (positions >= n_prompt-1); prefill_ms the prompt segment.  n_total <= min(max_seq_len, block_size) + 1. */
 int nb200_decode_greedy(nb200_engine *e, uint32_t *ids, uint32_t n_prompt, uint32_t n_total,
                         float repetition_penalty, float *prefill_ms, float *device_ms);
+
+/* Batched prompt prefill (no reference counterpart: infer.c:1146-1149 runs the prompt token by token and discards the logits).
+ * `ids` is the caller's output_ids array, as for nb200_next_greedy.  Runs the causal forward pass of ids[pos0 .. pos0+n) at
+ * positions pos0 .. pos0+n-1 in chunks of up to 16 positions per pass over the
+ * weights (nb200_config.reserved[5] reports the chunk size after the first call) and writes their K/V rows; no classifier, no
+ * logits, no state besides those rows.  The session then continues with nb200_forward / nb200_next_greedy / nb200_next_sampled
+ * at pos0+n, on either execution path.  The K/V rows are bit-identical to what nb200_forward at the same positions writes on
+ * the multi-kernel path (NB200_FLAG_NO_STREAM) of an engine created with the same flags; in exact mode that is the strict
+ * reference.  Rows outside [pos0, pos0+n) are not touched.  device_ms (optional): CUDA-event time of the call.
+ * NB200_EINVAL, with nothing written: n == 0, pos0 + n > min(max_seq_len, block_size), an id >= vocab_size, a tensor-parallel
+ * engine, an active LoRA plug-in.
+ * Not covered: the streaming kernel's own prompt loop (nb200_decode_greedy and the shim keep running the prompt token by token,
+ * so their fast-mode K/V bits do not change), tensor cores, non-causal (seq2seq) attention. */
+int nb200_prefill(nb200_engine *e, const uint32_t *ids, uint32_t pos0, uint32_t n, float *device_ms);
 
 /* introspection for parity tests */
 int nb200_read_buffer(nb200_engine *e, int field, uint32_t layer, uint32_t pos, float *dst, uint32_t count);

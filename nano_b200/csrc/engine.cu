@@ -27,6 +27,7 @@
 
 #include "../../include/nano_b200.h"
 #include "kernels.cuh"
+#include "prefill.cuh"
 #include "stream_host.h"
 #include "sample_host.h"
 
@@ -112,6 +113,7 @@ struct nb200_engine {
     uint64_t launches = 0, weight_bytes = 0;
     uint32_t launches_per_token = 0;
     uint32_t mv_mask = 0, attn_kind = 0;      // multi-kernel variants launched or captured so far (nb200_config.reserved[3], [4])
+    bool generic_attn = false;                // NB200_GENERIC_ATTN at creation: the generic attention kernel on every shape (tests)
     std::vector<uint32_t> seen_mirror;   // ids whose seen[] flag is set, by position
     bool seen_valid = false;
     std::vector<void *> allocs;
@@ -132,6 +134,14 @@ struct nb200_engine {
     bool prof_on = false; int prof_tag = 0;
     struct ProfRec { int tag; cudaEvent_t a, b; };
     std::vector<ProfRec> prof;
+    // batched prompt prefill (nb200_prefill, prefill.cuh): chunk size M and per-position buffers for M positions, allocated on the
+    // first call; attn_kind: the attention kernel of the last prefill (nb200_config.reserved[6])
+    struct Prefill {
+        uint32_t M = 0, attn_kind = 0;
+        float *x = nullptr, *q = nullptr, *kraw = nullptr, *xba = nullptr, *hb = nullptr;
+        float *ws_m = nullptr, *ws_l = nullptr, *ws_acc = nullptr, *att = nullptr;
+        uint32_t *tickets = nullptr, *ids = nullptr;
+    } pf;
 };
 
 namespace {
@@ -290,6 +300,15 @@ int run_embed(nb200_engine *e) {
     return launch<EmbedArgs>(e, k_embed, dim3(1), dim3(256), 0, a);
 }
 
+// fast mode: kv_mul when the split-KV attention specialised for it serves this shape, 0 for the generic k_attention
+// (NB200_GENERIC_ATTN at engine creation forces the generic kernel on one GPU)
+uint32_t fast_attn_kvm(const nb200_engine *e) {
+    const Dims &d = e->d;
+    const bool tp = e->tp_size > 1;
+    if (d.hd > 128 || (d.arch == 3u && (d.hd & (d.hd - 1)) != 0) || (!tp && e->generic_attn)) return 0;
+    return (d.kv_mul == 1 || d.kv_mul == 2 || d.kv_mul == 4 || d.kv_mul == 8) ? d.kv_mul : 0;
+}
+
 int run_layer(nb200_engine *e, uint32_t l) {
     const Dims &d = e->d;
     const size_t kvl = (size_t)d.KV * d.max_seq * d.hd;
@@ -330,7 +349,7 @@ int run_layer(nb200_engine *e, uint32_t l) {
         uint32_t smem = e->attn_smem;
         const bool tp = e->tp_size > 1;
         if (tp) a.tp = tp_args(e, 0, 4 * l + 1, e->tp_rank * d.q_dim, e->tp_off_xba);
-        if (d.hd <= 128 && (d.arch != 3u || (d.hd & (d.hd - 1)) == 0) && (tp || !getenv("NB200_GENERIC_ATTN"))) {
+        if (fast_attn_kvm(e)) {
             switch (d.kv_mul) {
                 case 1: kern = tp ? k_attention_fast<1, true> : k_attention_fast<1>; break;
                 case 2: kern = tp ? k_attention_fast<2, true> : k_attention_fast<2>; break;
@@ -408,6 +427,131 @@ int run_token(nb200_engine *e) {
     if ((r = run_embed(e))) return r;
     for (uint32_t l = 0; l < e->d.L; l++) if ((r = run_layer(e, l))) return r;
     return run_classifier(e);
+}
+
+// ---------------- batched prompt prefill (prefill.cuh) ----------------
+// Chunk size M: the largest value <= kPrefillMax for which M activation operands of the widest matrix, plus the prep's staging
+// copies, fit the shared memory one CTA can get.  The per-position buffers are allocated for M positions on the first call.
+int prefill_setup(nb200_engine *e) {
+    auto &pf = e->pf;
+    if (pf.M) return 0;
+    const Dims &d = e->d;
+    int optin = 0;
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->device));
+    uint32_t maxn = d.E; if (d.q_dim > maxn) maxn = d.q_dim; if (d.F > maxn) maxn = d.F;
+    const uint32_t widest = act_region_bytes(d.quant, maxn, d.gs ? d.gs : 1), stage = 2u * maxn * 4u;
+    const uint32_t budget = (uint32_t)optin - 256u;        // the kernels' static shared memory (reduction scratch) is 128 bytes
+    uint32_t M = kPrefillMax;
+    while (M > 0 && M * widest + stage > budget) M--;
+    if (!M) return fail(NB200_EINVAL, "prefill: one activation operand of %u elements does not fit in shared memory", maxn);
+    const size_t slots = (size_t)M * d.H * e->nsplit_max;
+    DM(pf.x, (size_t)M * d.E * 4); DM(pf.q, (size_t)M * d.q_dim * 4); DM(pf.kraw, (size_t)M * d.kv_dim * 4);
+    DM(pf.xba, (size_t)M * d.q_dim * 4); DM(pf.hb, (size_t)M * d.F * 4);
+    DM(pf.ws_m, slots * 4); DM(pf.ws_l, slots * 4); DM(pf.ws_acc, slots * d.hd * 4);
+    DM(pf.tickets, (size_t)M * d.KV * 4); CK(cudaMemset(pf.tickets, 0, (size_t)M * d.KV * 4));     // the merging CTA re-zeroes its ticket
+    if (d.exact) DM(pf.att, (size_t)M * d.H * d.max_seq * 4);
+    DM(pf.ids, (size_t)d.max_seq * 4);
+    pf.M = M;
+    return 0;
+}
+
+typedef void (*PrefillMvKern)(const PrefillMvArgs);
+
+template <int EPI>
+PrefillMvKern prefill_matvec_kernel(const Dims &d) {
+    constexpr int RB = kPrefillRB;
+    if (d.quant == 0x00u) return d.exact ? k_prefill_matvec_f32_exact<EPI> : k_prefill_matvec<0x00, EPI, RB, 8>;
+    if (d.quant == 0x42u) return k_prefill_matvec<0x42, EPI, RB, 8>;
+    switch (d.gs) {
+        case 32: return k_prefill_matvec<0x80, EPI, RB, 2>;
+        case 64: return k_prefill_matvec<0x80, EPI, RB, 4>;
+        case 128: return k_prefill_matvec<0x80, EPI, RB, 8>;
+        case 256: return k_prefill_matvec<0x80, EPI, RB, 16>;
+        default: return nullptr;
+    }
+}
+
+// one prefill matvec over the chunk: src / out rows of the m positions are `stride` floats apart
+int run_prefill_matvec(nb200_engine *e, int epi, const Mat &mt, PrefillMvArgs a) {
+    const Dims &d = e->d;
+    a.w = mt.w; a.w_aux = mt.aux; a.rows = mt.rows; a.n = mt.n; a.d = d;
+    a.act_bytes = act_region_bytes(d.quant, mt.n, d.gs ? d.gs : 1);
+    const uint32_t smem = a.m * a.act_bytes + 2u * mt.n * 4u;
+    PrefillMvKern k = nullptr;
+    switch (epi) {
+        case EPI_QKV: k = prefill_matvec_kernel<EPI_QKV>(d); break;
+        case EPI_RESID: k = prefill_matvec_kernel<EPI_RESID>(d); break;
+        case EPI_SWIGLU: k = prefill_matvec_kernel<EPI_SWIGLU>(d); break;
+    }
+    if (!k) return fail(NB200_EINVAL, "no prefill matvec kernel for quant=0x%x gs=%u", d.quant, d.gs);
+    uint32_t grid;
+    if (d.quant == 0x00u && d.exact) grid = ((epi == EPI_SWIGLU ? mt.rows / 2 : mt.rows) + kThreads - 1) / kThreads;
+    else grid = ((mt.rows + kPrefillRB - 1) / kPrefillRB + kWarps - 1) / kWarps;
+    if (grid > (uint32_t)e->num_sms) grid = (uint32_t)e->num_sms;
+    return launch<PrefillMvArgs>(e, k, dim3(grid), dim3(kThreads), smem, a);
+}
+
+// positions pos0 .. pos0+m-1 (m <= M), ids already on the device
+int run_prefill_chunk(nb200_engine *e, uint32_t pos0, uint32_t m, const uint32_t *ids) {
+    const Dims &d = e->d;
+    auto &pf = e->pf;
+    const size_t kvl = (size_t)d.KV * d.max_seq * d.hd;
+    const uint32_t kvm = d.exact ? 0u : fast_attn_kvm(e);
+    int r;
+    {
+        PrefillEmbedArgs a{e->emb.w, e->emb.aux, pf.x, ids, d};
+        if ((r = launch<PrefillEmbedArgs>(e, k_prefill_embed, dim3(m), dim3(256), 0, a))) return r;
+    }
+    for (uint32_t l = 0; l < d.L; l++) {
+        PrefillMvArgs a{};
+        a.pos0 = pos0; a.m = m;
+        a.src = pf.x; a.src_stride = d.E; a.gain = e->norm_attn + (size_t)l * d.E;
+        a.out = pf.q; a.out_stride = d.q_dim; a.out_k = pf.kraw; a.k_stride = d.kv_dim; a.out_v = e->vc + l * kvl;
+        if ((r = run_prefill_matvec(e, EPI_QKV, e->qkv[l], a))) return r;
+
+        const float *knorm = e->knorm ? e->knorm + (size_t)l * d.hd : nullptr;
+        PrefillKrowArgs kr{pf.kraw, e->kc + l * kvl, knorm, e->rope_cos, e->rope_sin, pos0, kvm ? 1u : 0u, d};
+        if ((r = launch<PrefillKrowArgs>(e, k_prefill_krow, dim3(d.KV, m), dim3(32), 0, kr))) return r;
+
+        PrefillAttnArgs pa{};
+        pa.pos0 = pos0;
+        if (d.exact) {
+            AttnExactArgs &x = pa.ex;
+            x.q = pf.q; x.kraw = pf.kraw; x.kc = e->kc + l * kvl; x.vc = e->vc + l * kvl;
+            x.qnorm = e->qnorm ? e->qnorm + (size_t)l * d.hd : nullptr; x.knorm = knorm;
+            x.rope_cos = e->rope_cos; x.rope_sin = e->rope_sin; x.xba = pf.xba; x.att = pf.att; x.d = d;
+            pf.attn_kind = 1u;
+            if ((r = launch<PrefillAttnArgs>(e, k_prefill_attention_exact, dim3(d.H, m), dim3(kAttnThreads), 2 * d.hd * 4, pa))) return r;
+        } else {
+            AttnArgs &at = pa.at;
+            at.q = pf.q; at.kraw = pf.kraw; at.kc = e->kc + l * kvl; at.vc = e->vc + l * kvl;
+            at.qnorm = e->qnorm ? e->qnorm + (size_t)l * d.hd : nullptr; at.knorm = knorm;
+            at.rope_cos = e->rope_cos; at.rope_sin = e->rope_sin; at.xba = pf.xba;
+            at.ws_m = pf.ws_m; at.ws_l = pf.ws_l; at.ws_acc = pf.ws_acc; at.ticket = pf.tickets;
+            at.nsplit_max = e->nsplit_max; at.chunk_cap = e->chunk_cap; at.d = d;
+            void (*kern)(const PrefillAttnArgs) = k_prefill_attention;
+            switch (kvm) {
+                case 1: kern = k_prefill_attention_fast<1>; break;
+                case 2: kern = k_prefill_attention_fast<2>; break;
+                case 4: kern = k_prefill_attention_fast<4>; break;
+                case 8: kern = k_prefill_attention_fast<8>; break;
+                default: break;
+            }
+            const uint32_t smem = kvm ? attn_fast_smem_floats(d.kv_mul, d.hd, e->chunk_cap, e->nsplit_max, kWarps) * 4u : e->attn_smem;
+            pf.attn_kind = kvm ? (3u | (kvm << 8)) : 2u;
+            if ((r = launch<PrefillAttnArgs>(e, kern, dim3(e->nsplit_max, d.KV, m), dim3(kvm ? kThreads : kAttnThreads), smem, pa))) return r;
+        }
+
+        a = PrefillMvArgs{};
+        a.pos0 = pos0; a.m = m;
+        a.src = pf.xba; a.src_stride = d.q_dim; a.out = pf.x; a.out_stride = d.E;
+        if ((r = run_prefill_matvec(e, EPI_RESID, e->wo[l], a))) return r;
+        a.src = pf.x; a.src_stride = d.E; a.gain = e->norm_ffn + (size_t)l * d.E; a.out = pf.hb; a.out_stride = d.F;
+        if ((r = run_prefill_matvec(e, EPI_SWIGLU, e->w13[l], a))) return r;
+        a.src = pf.hb; a.src_stride = d.F; a.gain = nullptr; a.out = pf.x; a.out_stride = d.E;
+        if ((r = run_prefill_matvec(e, EPI_RESID, e->w2[l], a))) return r;
+    }
+    return 0;
 }
 
 // n_steps tokens in ONE cooperative launch of the streaming kernel
@@ -705,6 +849,7 @@ static int create_impl(nb200_engine **out, const uint8_t *img, uint64_t image_by
     struct Guard { nb200_engine *e; bool ok = false; ~Guard() { if (!ok) nb200_engine_destroy(e); } } guard{e};
     e->device = device; e->flags = flags; e->tp_rank = tp_rank; e->tp_size = tp_size;
     e->use_pdl = !(flags & NB200_FLAG_NO_PDL);
+    e->generic_attn = getenv("NB200_GENERIC_ATTN") != nullptr;
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
     e->num_sms = prop.multiProcessorCount;
@@ -1163,6 +1308,8 @@ int nb200_get_config(const nb200_engine *e, nb200_config *c) {
     c->reserved[2] = (uint32_t)(e->calib_ms[1] * 1000.0f + 0.5f);     // ... and of the multi-kernel graph (0 = the choice was not measured)
     c->reserved[3] = e->mv_mask;
     c->reserved[4] = e->attn_kind;
+    c->reserved[5] = e->pf.M;                 // nb200_prefill: positions per chunk (0 until the first call)
+    c->reserved[6] = e->pf.attn_kind;         // ... and its attention kernel, encoded as [4]
     return 0;
 }
 
@@ -1294,6 +1441,33 @@ int nb200_decode_greedy(nb200_engine *e, uint32_t *ids, uint32_t n_prompt, uint3
     if (prefill_ms) *prefill_ms = a;
     if (device_ms) *device_ms = b;
     return tp_check(e);
+}
+
+int nb200_prefill(nb200_engine *e, const uint32_t *ids, uint32_t pos0, uint32_t n, float *device_ms) {
+    if (!e || !ids) return fail(NB200_EINVAL, "null argument");
+    if (e->tp_size > 1) return fail(NB200_EINVAL, "prefill is not available on tensor-parallel engines");
+    if (e->lora.active) return fail(NB200_EINVAL, "prefill does not run LoRA plug-ins: disable the plug-in (nb200_lora_enable) or use nb200_forward");
+    const uint32_t lim = pos_limit(e->d);
+    if (n == 0 || pos0 >= lim || n > lim - pos0)
+        return fail(NB200_EINVAL, "prefill of %u positions from %u: empty, or past min(max_seq_len, block_size) = %u", n, pos0, lim);
+    for (uint32_t p = pos0; p < pos0 + n; p++) if (ids[p] >= e->d.V) return fail(NB200_EINVAL, "id %u at position %u out of range", ids[p], p);
+    CK(cudaSetDevice(e->device));
+    int r;
+    if ((r = prefill_setup(e))) return r;
+    struct Events { cudaEvent_t ev[2] = {nullptr, nullptr}; ~Events() { for (auto v : ev) if (v) cudaEventDestroy(v); } } evs;
+    for (auto &v : evs.ev) CK(cudaEventCreate(&v));
+    CK(cudaMemcpyAsync(e->pf.ids, ids + pos0, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaEventRecord(evs.ev[0], e->stream));
+    for (uint32_t c = 0; c < n; c += e->pf.M) {
+        const uint32_t m = (n - c < e->pf.M) ? n - c : e->pf.M;
+        if ((r = run_prefill_chunk(e, pos0 + c, m, e->pf.ids + c))) return r;
+    }
+    CK(cudaEventRecord(evs.ev[1], e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    float ms = 0.0f;
+    CK(cudaEventElapsedTime(&ms, evs.ev[0], evs.ev[1]));
+    if (device_ms) *device_ms = ms;
+    return 0;
 }
 
 int nb200_read_buffer(nb200_engine *e, int field, uint32_t layer, uint32_t pos, float *dst, uint32_t count) {

@@ -1539,19 +1539,13 @@ __global__ void __launch_bounds__(kThreads) k_attention_fast(const AttnArgs a) {
     attn_item<KVM, kThreads, TP>(a, blockIdx.y, blockIdx.x, pos, range, chunk, nsplit, sm, is_last);
 }
 
-NB_K __global__ void __launch_bounds__(kAttnThreads) k_attention(const AttnArgs a) {
-    extern __shared__ __align__(16) float sm[];
-    __shared__ float red[32];
-    __shared__ uint32_t is_last;
-    pdl_launch_dependents();
-    pdl_wait();
-
+// One (kv head g, split) CTA of the generic split-KV attention for the position `pos` attending to rows [0, range).
+// k_attention runs it for the step's position; k_prefill_attention (prefill.cuh) for each position of a prompt chunk.
+__device__ __forceinline__ void attn_generic_cta(const AttnArgs &a, uint32_t g, uint32_t split, uint32_t pos, uint32_t range,
+                                                 float *sm, float *red, uint32_t &is_last) {
     const Dims &d = a.d;
     const bool exact = d.exact != 0;
     const uint32_t hd = d.hd, kvm = d.kv_mul;
-    const uint32_t g = blockIdx.y, split = blockIdx.x;
-    const uint32_t pos = a.st->pos;
-    const uint32_t range = a.st->is_causal ? pos + 1 : d.max_seq;
     uint32_t chunk = (range + a.nsplit_max - 1) / a.nsplit_max;
     chunk = max(chunk, 32u);
     chunk = min((chunk + 7u) & ~7u, a.chunk_cap);
@@ -1681,6 +1675,17 @@ NB_K __global__ void __launch_bounds__(kAttnThreads) k_attention(const AttnArgs 
     if (threadIdx.x == 0) a.ticket[g] = 0;
 }
 
+NB_K __global__ void __launch_bounds__(kAttnThreads) k_attention(const AttnArgs a) {
+    extern __shared__ __align__(16) float sm[];
+    __shared__ float red[32];
+    __shared__ uint32_t is_last;
+    pdl_launch_dependents();
+    pdl_wait();
+    const uint32_t pos = a.st->pos;
+    const uint32_t range = a.st->is_causal ? pos + 1 : a.d.max_seq;
+    attn_generic_cta(a, blockIdx.y, blockIdx.x, pos, range, sm, red, is_last);
+}
+
 // exact-mode attention: one CTA per q head, the reference's loop order (infer.c:841-879).
 // att: [H][max_seq] scratch in HBM.
 struct AttnExactArgs {
@@ -1688,15 +1693,10 @@ struct AttnExactArgs {
     float *xba; float *att; const DevState *st; Dims d;
 };
 
-NB_K __global__ void __launch_bounds__(kAttnThreads) k_attention_exact(const AttnExactArgs a) {
-    extern __shared__ __align__(16) float sm[];
-    __shared__ float red[32];
-    pdl_launch_dependents();
-    pdl_wait();
+// the CTA of q head h for the position `pos` attending to rows [0, range) (k_attention_exact; k_prefill_attention_exact)
+__device__ __forceinline__ void attn_exact_cta(const AttnExactArgs &a, uint32_t h, uint32_t pos, uint32_t range, float *sm, float *red) {
     const Dims &d = a.d;
-    const uint32_t hd = d.hd, h = blockIdx.x, g = h / d.kv_mul;
-    const uint32_t pos = a.st->pos;
-    const uint32_t range = a.st->is_causal ? pos + 1 : d.max_seq;
+    const uint32_t hd = d.hd, g = h / d.kv_mul;
     float *qs = sm, *krow = sm + hd;
     const int warp = threadIdx.x >> 5;
     const float *cr = a.rope_cos + (size_t)pos * (hd / 2), *ci = a.rope_sin + (size_t)pos * (hd / 2);
@@ -1738,6 +1738,16 @@ NB_K __global__ void __launch_bounds__(kAttnThreads) k_attention_exact(const Att
         }
         a.xba[(size_t)h * hd + i] = o;
     }
+}
+
+NB_K __global__ void __launch_bounds__(kAttnThreads) k_attention_exact(const AttnExactArgs a) {
+    extern __shared__ __align__(16) float sm[];
+    __shared__ float red[32];
+    pdl_launch_dependents();
+    pdl_wait();
+    const uint32_t pos = a.st->pos;
+    const uint32_t range = a.st->is_causal ? pos + 1 : a.d.max_seq;
+    attn_exact_cta(a, blockIdx.x, pos, range, sm, red);
 }
 
 // penalty + first-max argmax + state update over logits already in HBM (exact-mode F32 classifier)

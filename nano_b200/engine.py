@@ -24,7 +24,8 @@ MATVEC_EPILOGUES = ("store", "qkv", "resid", "swiglu", "cls")      # kernels.cuh
 
 EXPORTS = [
     "nb200_last_error", "nb200_device_count", "nb200_engine_create", "nb200_engine_destroy", "nb200_get_config",
-    "nb200_forward", "nb200_read_logits", "nb200_next_greedy", "nb200_next_sampled", "nb200_decode_greedy", "nb200_read_buffer",
+    "nb200_forward", "nb200_read_logits", "nb200_next_greedy", "nb200_next_sampled", "nb200_decode_greedy", "nb200_prefill",
+    "nb200_read_buffer",
     "nb200_write_x", "nb200_run_layer", "nb200_profile_tokens", "nb200_trace_token", "nb200_read_attn_trace", "nb200_kernel_launches", "nb200_launches_per_token", "nb200_weight_bytes",
     "nb200_op_rmsnorm", "nb200_op_q80_quantize", "nb200_op_q80_matvec", "nb200_op_f32_matvec",
     "nb200_op_q4k_quantize", "nb200_op_q4k_matvec",
@@ -69,6 +70,7 @@ def lib():
         L.nb200_next_greedy.argtypes = [C.c_void_p, u32p, C.c_uint32, C.c_int, C.c_float, u32p]
         L.nb200_next_sampled.argtypes = [C.c_void_p, u32p, C.c_uint32, C.c_float, C.c_float, C.c_float, C.c_float, u32p, u32p]
         L.nb200_decode_greedy.argtypes = [C.c_void_p, u32p, C.c_uint32, C.c_uint32, C.c_float, f32p, f32p]
+        L.nb200_prefill.argtypes = [C.c_void_p, u32p, C.c_uint32, C.c_uint32, f32p]
         L.nb200_read_buffer.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32]
         L.nb200_write_x.argtypes = [C.c_void_p, f32p, C.c_uint32]
         L.nb200_run_layer.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]
@@ -112,6 +114,10 @@ def _p(a: np.ndarray, t):
     return a.ctypes.data_as(t)
 
 
+def _attention_kind(att: int):
+    return {0: None, 1: "exact", 2: "generic", 3: f"fast<{att >> 8}>"}[att & 0xff]
+
+
 class Engine:
     """One model resident in the HBM of one GPU."""
 
@@ -152,8 +158,14 @@ class Engine:
         _check(lib().nb200_get_config(self.h, C.byref(cfg)))
         mask, att = int(cfg.reserved[3]), int(cfg.reserved[4])
         mv = {(epi, rb) for i, epi in enumerate(MATVEC_EPILOGUES) for j, rb in enumerate((1, 2, 4)) if mask >> (3 * i + j) & 1}
-        kind = {0: None, 1: "exact", 2: "generic", 3: f"fast<{att >> 8}>"}[att & 0xff]
-        return {"matvec": mv, "attention": kind}
+        return {"matvec": mv, "attention": _attention_kind(att)}
+
+    def prefill_info(self) -> dict:
+        """Batched prefill (reserved[5] / [6]): {"chunk": positions per pass over the weights (0 before the first prefill),
+        "attention": the attention kernel of the last prefill, named as in kernels()}."""
+        cfg = Config()
+        _check(lib().nb200_get_config(self.h, C.byref(cfg)))
+        return {"chunk": int(cfg.reserved[5]), "attention": _attention_kind(int(cfg.reserved[6]))}
 
     # ---- LoRA plug-in ----
     def lora_load(self, image: bytes) -> None:
@@ -228,6 +240,15 @@ class Engine:
         a, b = C.c_float(0), C.c_float(0)
         _check(lib().nb200_decode_greedy(self.h, _p(ids, u32p), n_prompt, n_total, penalty, C.byref(a), C.byref(b)))
         return float(a.value), float(b.value)
+
+    def prefill(self, ids: np.ndarray, pos0: int, n: int) -> float:
+        """Batched prompt prefill of ids[pos0:pos0+n] at positions pos0.. (K/V rows only; continue with forward / next_greedy /
+        next_sampled at pos0+n).  Returns the device time in ms."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint32)
+        assert ids.size >= pos0 + n
+        ms = C.c_float(0)
+        _check(lib().nb200_prefill(self.h, _p(ids, u32p), int(pos0), int(n), C.byref(ms)))
+        return float(ms.value)
 
     def read(self, field: int, count: int, layer: int = 0, pos: int = 0, dtype=np.float32) -> np.ndarray:
         out = np.zeros(count, dtype=dtype)
