@@ -77,6 +77,15 @@ __global__ void k_q4k_split(const uint8_t *__restrict__ blocks, uint64_t nblocks
     }
 }
 
+// Per-layer activations and attention workspaces for m positions (the token path: 1, prefill: M); position p's rows follow
+// position p-1's.  On tensor-parallel engines the token path's x / xba / hb live in the exchange block.
+struct LayerBufs {
+    float *x = nullptr, *q = nullptr, *kraw = nullptr, *xba = nullptr, *hb = nullptr;
+    float *ws_m = nullptr, *ws_l = nullptr, *ws_acc = nullptr;      // split-KV partials [m][H][nsplit_max] ([..][hd])
+    uint32_t *tickets = nullptr;                                    // [m][KV]
+    float *att = nullptr;                                           // exact mode: scores [m][H][max_seq]
+};
+
 }  // namespace
 
 struct nb200_engine {
@@ -88,10 +97,9 @@ struct nb200_engine {
     Mat cls, emb;
     float *norm_attn = nullptr, *norm_ffn = nullptr, *norm_final = nullptr, *qnorm = nullptr, *knorm = nullptr;
     float *rope_cos = nullptr, *rope_sin = nullptr;
-    float *x = nullptr, *q = nullptr, *kraw = nullptr, *xba = nullptr, *hb = nullptr, *logits = nullptr;
-    float *kc = nullptr, *vc = nullptr, *att_exact = nullptr;
-    float *ws_m = nullptr, *ws_l = nullptr, *ws_acc = nullptr;
-    uint32_t *tickets = nullptr, *ids_dev = nullptr, *cls_idx = nullptr;
+    LayerBufs buf;                    // the token path's
+    float *logits = nullptr, *kc = nullptr, *vc = nullptr;
+    uint32_t *ids_dev = nullptr, *cls_idx = nullptr;
     float *cls_val = nullptr;
     uint8_t *seen = nullptr;
     DevState *st = nullptr;
@@ -138,9 +146,8 @@ struct nb200_engine {
     // first call; attn_kind: the attention kernel of the last prefill (nb200_config.reserved[6])
     struct Prefill {
         uint32_t M = 0, attn_kind = 0;
-        float *x = nullptr, *q = nullptr, *kraw = nullptr, *xba = nullptr, *hb = nullptr;
-        float *ws_m = nullptr, *ws_l = nullptr, *ws_acc = nullptr, *att = nullptr;
-        uint32_t *tickets = nullptr, *ids = nullptr;
+        LayerBufs buf;
+        uint32_t *ids = nullptr;
     } pf;
 };
 
@@ -154,6 +161,20 @@ int dmalloc(nb200_engine *e, void **p, size_t bytes) {
     return 0;
 }
 #define DM(ptr, bytes) do { int r_ = dmalloc(e, (void **)&(ptr), (bytes)); if (r_) return r_; } while (0)
+
+// b's buffers for m positions; x / xba / hb only where not set already (the exchange block of a tensor-parallel engine)
+int alloc_layer_bufs(nb200_engine *e, LayerBufs &b, uint32_t m) {
+    const Dims &d = e->d;
+    const size_t slots = (size_t)m * d.H * e->nsplit_max;
+    if (!b.x) DM(b.x, (size_t)m * d.E * 4);
+    if (!b.xba) DM(b.xba, (size_t)m * d.q_dim * 4);
+    if (!b.hb) DM(b.hb, (size_t)m * d.F * 4);
+    DM(b.q, (size_t)m * d.q_dim * 4); DM(b.kraw, (size_t)m * d.kv_dim * 4);
+    DM(b.ws_m, slots * 4); DM(b.ws_l, slots * 4); DM(b.ws_acc, slots * d.hd * 4);
+    DM(b.tickets, (size_t)m * d.KV * 4); CK(cudaMemset(b.tickets, 0, (size_t)m * d.KV * 4));     // the merging CTA re-zeroes its ticket
+    if (d.exact) DM(b.att, (size_t)m * d.H * d.max_seq * 4);
+    return 0;
+}
 
 // ---------------- kernel launch plumbing ----------------
 template <typename Args>
@@ -223,12 +244,14 @@ int grid_mult() {
     return m;
 }
 
+// Q80 lanes per group of the matvec kernels (a 16-byte code slice per lane); F32 and Q4K kernels are instantiated at 8
+int matvec_lpg(const Dims &d) { return (d.quant == 0x80u) ? (int)(d.gs / 16) : 8; }
+
 // one fused matvec launch
-int run_matvec(nb200_engine *e, int epi, const Mat &m, MatvecArgs a, bool norm, int num_sms) {
+int run_matvec(nb200_engine *e, int epi, const Mat &m, MatvecArgs a, int num_sms) {
     const Dims &d = a.d;
     a.w = m.w; a.w_aux = m.aux; a.rows = m.rows; a.n = m.n;
     const uint32_t smem = act_smem_bytes(d.quant, m.n, d.gs ? d.gs : 1);
-    (void)norm;
     if (d.quant == 0x00u && d.exact) {
         MatvecKern k = nullptr;
         switch (epi) {
@@ -256,7 +279,7 @@ int run_matvec(nb200_engine *e, int epi, const Mat &m, MatvecArgs a, bool norm, 
         if (want == 2 || want == 4) rb = want;
         else if (want == 1) rb = (d.quant == 0x80u && epi != EPI_SWIGLU) ? 1 : 2;
     }
-    const int lpg = (d.quant == 0x80u) ? (int)(d.gs / 16) : 8;
+    const int lpg = matvec_lpg(d);
     MatvecKern k = nullptr;
     const bool tp = a.tp.size > 1;
     switch (epi) {
@@ -295,85 +318,97 @@ TpArgs tp_args(nb200_engine *e, uint32_t wait_ph, uint32_t signal_ph, uint32_t r
 
 int run_embed(nb200_engine *e) {
     EmbedArgs a{};
-    a.w = e->emb.w; a.w_aux = e->emb.aux; a.x = e->x; a.ids = e->ids_dev; a.st = e->st; a.d = e->d; a.ll = e->tp_size > 1;
+    a.w = e->emb.w; a.w_aux = e->emb.aux; a.x = e->buf.x; a.ids = e->ids_dev; a.st = e->st; a.d = e->d; a.ll = e->tp_size > 1;
     e->prof_tag = 0;
     return launch<EmbedArgs>(e, k_embed, dim3(1), dim3(256), 0, a);
 }
 
-// fast mode: kv_mul when the split-KV attention specialised for it serves this shape, 0 for the generic k_attention
-// (NB200_GENERIC_ATTN at engine creation forces the generic kernel on one GPU)
-uint32_t fast_attn_kvm(const nb200_engine *e) {
+// The attention kernel of an engine, in its token-path and prefill variants: exact (k_attention_exact has its own
+// argument type, so `tok` is unset), fast<KVM> where the split-KV attention specialised for kv_mul serves the shape, else
+// the generic kernel (on one GPU also under NB200_GENERIC_ATTN at engine creation).
+struct AttnChoice {
+    void (*tok)(const AttnArgs);
+    void (*pf)(const PrefillAttnArgs);
+    uint32_t threads, smem;
+    uint32_t kvm;       // fast<KVM>: kv_mul; generic and exact: 0
+    uint32_t kind;      // nb200_config.reserved[4] / [6]: 1 exact, 2 generic, 3 | kv_mul << 8 fast
+};
+
+AttnChoice pick_attn(const nb200_engine *e) {
     const Dims &d = e->d;
+    if (d.exact) return {nullptr, k_prefill_attention_exact, kAttnThreads, 2 * d.hd * 4, 0u, 1u};
     const bool tp = e->tp_size > 1;
-    if (d.hd > 128 || (d.arch == 3u && (d.hd & (d.hd - 1)) != 0) || (!tp && e->generic_attn)) return 0;
-    return (d.kv_mul == 1 || d.kv_mul == 2 || d.kv_mul == 4 || d.kv_mul == 8) ? d.kv_mul : 0;
+    if (d.hd <= 128 && !(d.arch == 3u && (d.hd & (d.hd - 1)) != 0) && (tp || !e->generic_attn)) {
+        const uint32_t smem = attn_fast_smem_floats(d.kv_mul, d.hd, e->chunk_cap, e->nsplit_max, kWarps) * 4u;
+        switch (d.kv_mul) {
+#define NB_FAST(K) case K: return {tp ? k_attention_fast<K, true> : k_attention_fast<K>, k_prefill_attention_fast<K>, kThreads, smem, K, 3u | (K << 8)};
+            NB_FAST(1) NB_FAST(2) NB_FAST(4) NB_FAST(8)
+#undef NB_FAST
+            default: break;
+        }
+    }
+    return {k_attention, k_prefill_attention, kAttnThreads, e->attn_smem, 0u, 2u};
+}
+
+// the attention arguments of layer l over the buffers b (position 0 of b): the split-KV kernels' and the exact kernel's
+void attn_args(const nb200_engine *e, const LayerBufs &b, uint32_t l, AttnArgs &at, AttnExactArgs &ex) {
+    const Dims &d = e->d;
+    const size_t kvl = (size_t)d.KV * d.max_seq * d.hd;
+    at = AttnArgs{};
+    at.q = b.q; at.kraw = b.kraw; at.kc = e->kc + l * kvl; at.vc = e->vc + l * kvl;
+    at.qnorm = e->qnorm ? e->qnorm + (size_t)l * d.hd : nullptr;
+    at.knorm = e->knorm ? e->knorm + (size_t)l * d.hd : nullptr;
+    at.rope_cos = e->rope_cos; at.rope_sin = e->rope_sin; at.xba = b.xba;
+    at.ws_m = b.ws_m; at.ws_l = b.ws_l; at.ws_acc = b.ws_acc; at.ticket = b.tickets;
+    at.st = e->st; at.nsplit_max = e->nsplit_max; at.chunk_cap = e->chunk_cap; at.d = d;
+    ex = AttnExactArgs{at.q, at.kraw, at.kc, at.vc, at.qnorm, at.knorm, at.rope_cos, at.rope_sin, at.xba, b.att, e->st, d};
 }
 
 int run_layer(nb200_engine *e, uint32_t l) {
     const Dims &d = e->d;
+    const LayerBufs &b = e->buf;
     const size_t kvl = (size_t)d.KV * d.max_seq * d.hd;
     int r;
     {   // F1: rmsnorm + quantise + QKV matvec + KV store
         MatvecArgs a = base_args(e);
-        a.src = e->x; a.gain = e->norm_attn + (size_t)l * d.E;
-        a.out = e->q; a.out_k = e->kraw; a.out_v = e->vc + l * kvl;
+        a.src = b.x; a.gain = e->norm_attn + (size_t)l * d.E;
+        a.out = b.q; a.out_k = b.kraw; a.out_v = e->vc + l * kvl;
         a.dump_codes = e->dump_codes; a.dump_scales = e->dump_scales;
         a.tp = tp_args(e, 4 * l, 0, 0, 0);
         e->prof_tag = 1;
-        if ((r = run_matvec(e, EPI_QKV, e->qkv[l], a, true, e->num_sms))) return r;
+        if ((r = run_matvec(e, EPI_QKV, e->qkv[l], a, e->num_sms))) return r;
     }
     if (e->lora.active) {   // q/k/v LoRA branches on xb = rmsnorm(x)*gain, added before RoPE (infer.c:792-808)
         const uint32_t rk = e->lora.rank;
         LoraAArgs la{};
-        la.src = e->x; la.gain = e->norm_attn + (size_t)l * d.E; la.n = d.E; la.nmat = 3; la.rank = rk; la.t = e->lora.t; la.exact = d.exact;
+        la.src = b.x; la.gain = e->norm_attn + (size_t)l * d.E; la.n = d.E; la.nmat = 3; la.rank = rk; la.t = e->lora.t; la.exact = d.exact;
         for (int m = 0; m < 3; m++) la.A[m] = e->lora.a[m] + (size_t)l * rk * d.E;
         if ((r = launch<LoraAArgs>(e, k_lora_a, dim3((3 * rk + kWarps - 1) / kWarps), dim3(kThreads), 3 * d.E * 4, la))) return r;
         LoraBArgs lb{};
         lb.t = e->lora.t; lb.nmat = 3; lb.rank = rk; lb.scale = (float)e->lora.alpha / (float)rk;
         lb.rows[0] = d.q_dim; lb.rows[1] = d.kv_dim; lb.rows[2] = d.kv_dim;
         lb.B[0] = e->lora.b[0] + (size_t)l * d.q_dim * rk; lb.B[1] = e->lora.b[1] + (size_t)l * d.kv_dim * rk; lb.B[2] = e->lora.b[2] + (size_t)l * d.kv_dim * rk;
-        lb.dst[0] = e->q; lb.dst[1] = e->kraw; lb.dst[2] = nullptr; lb.vcache = e->vc + l * kvl; lb.store = 0; lb.st = e->st; lb.d = d;
+        lb.dst[0] = b.q; lb.dst[1] = b.kraw; lb.dst[2] = nullptr; lb.vcache = e->vc + l * kvl; lb.store = 0; lb.st = e->st; lb.d = d;
         if ((r = launch<LoraBArgs>(e, k_lora_b, dim3((d.q_dim + 2 * d.kv_dim + 255) / 256), dim3(256), 0, lb))) return r;
     }
-    e->prof_tag = 2;
-    if (!d.exact) {   // F2: head-norm + RoPE + split-KV attention
-        AttnArgs a{};
-        a.q = e->q; a.kraw = e->kraw; a.kc = e->kc + l * kvl; a.vc = e->vc + l * kvl;
-        a.qnorm = e->qnorm ? e->qnorm + (size_t)l * d.hd : nullptr;
-        a.knorm = e->knorm ? e->knorm + (size_t)l * d.hd : nullptr;
-        a.rope_cos = e->rope_cos; a.rope_sin = e->rope_sin; a.xba = e->xba;
-        a.ws_m = e->ws_m; a.ws_l = e->ws_l; a.ws_acc = e->ws_acc; a.ticket = e->tickets;
-        a.st = e->st; a.nsplit_max = e->nsplit_max; a.chunk_cap = e->chunk_cap; a.d = d;
-        a.dbg = (l == d.L / 2) ? e->attn_dbg : nullptr;
-        void (*kern)(const AttnArgs) = k_attention;
-        uint32_t smem = e->attn_smem;
-        const bool tp = e->tp_size > 1;
-        if (tp) a.tp = tp_args(e, 0, 4 * l + 1, e->tp_rank * d.q_dim, e->tp_off_xba);
-        if (fast_attn_kvm(e)) {
-            switch (d.kv_mul) {
-                case 1: kern = tp ? k_attention_fast<1, true> : k_attention_fast<1>; break;
-                case 2: kern = tp ? k_attention_fast<2, true> : k_attention_fast<2>; break;
-                case 4: kern = tp ? k_attention_fast<4, true> : k_attention_fast<4>; break;
-                case 8: kern = tp ? k_attention_fast<8, true> : k_attention_fast<8>; break;
-                default: break;
-            }
-            if (kern != k_attention) smem = attn_fast_smem_floats(d.kv_mul, d.hd, e->chunk_cap, e->nsplit_max, kWarps) * 4u;
+    {   // F2: head-norm + RoPE + attention
+        e->prof_tag = 2;
+        const AttnChoice ac = pick_attn(e);
+        AttnArgs at; AttnExactArgs ex;
+        attn_args(e, b, l, at, ex);
+        e->attn_kind = ac.kind;
+        if (d.exact) r = launch<AttnExactArgs>(e, k_attention_exact, dim3(d.H), dim3(ac.threads), ac.smem, ex);
+        else {
+            at.dbg = (l == d.L / 2) ? e->attn_dbg : nullptr;
+            if (e->tp_size > 1) at.tp = tp_args(e, 0, 4 * l + 1, e->tp_rank * d.q_dim, e->tp_off_xba);
+            r = launch<AttnArgs>(e, ac.tok, dim3(e->nsplit_max, d.KV), dim3(ac.threads), ac.smem, at);
         }
-        e->attn_kind = (kern == k_attention) ? 2u : (3u | (d.kv_mul << 8));
-        if ((r = launch<AttnArgs>(e, kern, dim3(e->nsplit_max, d.KV), dim3(kern != k_attention ? kThreads : kAttnThreads), smem, a))) return r;
-    } else {
-        AttnExactArgs a{};
-        a.q = e->q; a.kraw = e->kraw; a.kc = e->kc + l * kvl; a.vc = e->vc + l * kvl;
-        a.qnorm = e->qnorm ? e->qnorm + (size_t)l * d.hd : nullptr;
-        a.knorm = e->knorm ? e->knorm + (size_t)l * d.hd : nullptr;
-        a.rope_cos = e->rope_cos; a.rope_sin = e->rope_sin; a.xba = e->xba; a.att = e->att_exact; a.st = e->st; a.d = d;
-        e->attn_kind = 1u;
-        if ((r = launch<AttnExactArgs>(e, k_attention_exact, dim3(d.H), dim3(kAttnThreads), 2 * d.hd * 4, a))) return r;
+        if (r) return r;
     }
     if (e->lora.active) {   // o branch on the attention output; added to the O result before the residual (infer.c:898-903)
         const uint32_t rk = e->lora.rank;
         LoraAArgs la{};
-        la.src = e->xba; la.gain = nullptr; la.n = d.q_dim; la.nmat = 1; la.rank = rk; la.t = e->lora.t + 3 * rk; la.exact = d.exact;
+        la.src = b.xba; la.gain = nullptr; la.n = d.q_dim; la.nmat = 1; la.rank = rk; la.t = e->lora.t + 3 * rk; la.exact = d.exact;
         la.A[0] = e->lora.a[3] + (size_t)l * rk * d.q_dim;
         e->prof_tag = 3;
         if ((r = launch<LoraAArgs>(e, k_lora_a, dim3((rk + kWarps - 1) / kWarps), dim3(kThreads), 3 * d.q_dim * 4, la))) return r;
@@ -384,25 +419,25 @@ int run_layer(nb200_engine *e, uint32_t l) {
     }
     {   // F3: quantise(xba) + O matvec + residual
         MatvecArgs a = base_args(e);
-        a.src = e->xba; a.gain = nullptr; a.out = e->x;
+        a.src = b.xba; a.gain = nullptr; a.out = b.x;
         a.lora_add = e->lora.active ? e->lora.o1 : nullptr;
         a.tp = tp_args(e, 4 * l + 1, 4 * l + 2, e->tp_rank * e->wo[l].rows, e->tp_off_x);
         e->prof_tag = 3;
-        if ((r = run_matvec(e, EPI_RESID, e->wo[l], a, false, e->num_sms))) return r;
+        if ((r = run_matvec(e, EPI_RESID, e->wo[l], a, e->num_sms))) return r;
     }
     {   // F4: rmsnorm + quantise + W1|W3 matvec + SwiGLU
         MatvecArgs a = base_args(e);
-        a.src = e->x; a.gain = e->norm_ffn + (size_t)l * d.E; a.out = e->hb;
+        a.src = b.x; a.gain = e->norm_ffn + (size_t)l * d.E; a.out = b.hb;
         a.tp = tp_args(e, 4 * l + 2, 4 * l + 3, e->tp_rank * (e->w13[l].rows / 2), e->tp_off_hb);
         e->prof_tag = 4;
-        if ((r = run_matvec(e, EPI_SWIGLU, e->w13[l], a, true, e->num_sms))) return r;
+        if ((r = run_matvec(e, EPI_SWIGLU, e->w13[l], a, e->num_sms))) return r;
     }
     {   // F5: quantise(hb) + W2 matvec + residual
         MatvecArgs a = base_args(e);
-        a.src = e->hb; a.gain = nullptr; a.out = e->x;
+        a.src = b.hb; a.gain = nullptr; a.out = b.x;
         a.tp = tp_args(e, 4 * l + 3, 4 * l + 4, e->tp_rank * e->w2[l].rows, e->tp_off_x);
         e->prof_tag = 5;
-        if ((r = run_matvec(e, EPI_RESID, e->w2[l], a, false, e->num_sms))) return r;
+        if ((r = run_matvec(e, EPI_RESID, e->w2[l], a, e->num_sms))) return r;
     }
     return 0;
 }
@@ -410,16 +445,16 @@ int run_layer(nb200_engine *e, uint32_t l) {
 int run_classifier(nb200_engine *e) {
     e->prof_tag = 6;
     MatvecArgs a = base_args(e);
-    a.src = e->x; a.gain = e->norm_final; a.out = e->logits;
+    a.src = e->buf.x; a.gain = e->norm_final; a.out = e->logits;
     if (e->d.quant == 0x00u && e->d.exact) {
-        int r = run_matvec(e, EPI_STORE, e->cls, a, true, e->num_sms);
+        int r = run_matvec(e, EPI_STORE, e->cls, a, e->num_sms);
         if (r) return r;
         FinalizeArgs f{e->logits, e->d.V, e->seen, e->seen, e->ids_dev, e->st};
         return launch<FinalizeArgs>(e, k_cls_finalize, dim3(1), dim3(1024), 0, f);
     }
     a.st_rw = e->st; a.seen = e->seen; a.seen_rw = e->seen; a.cls_val = e->cls_val; a.cls_idx = e->cls_idx; a.ids = e->ids_dev;
     a.tp = tp_args(e, 4 * e->d.L, 4 * e->d.L + 1, e->tp_rank * e->cls.rows, 0);
-    return run_matvec(e, EPI_CLS, e->cls, a, true, e->num_sms);
+    return run_matvec(e, EPI_CLS, e->cls, a, e->num_sms);
 }
 
 int run_token(nb200_engine *e) {
@@ -444,12 +479,8 @@ int prefill_setup(nb200_engine *e) {
     uint32_t M = kPrefillMax;
     while (M > 0 && M * widest + stage > budget) M--;
     if (!M) return fail(NB200_EINVAL, "prefill: one activation operand of %u elements does not fit in shared memory", maxn);
-    const size_t slots = (size_t)M * d.H * e->nsplit_max;
-    DM(pf.x, (size_t)M * d.E * 4); DM(pf.q, (size_t)M * d.q_dim * 4); DM(pf.kraw, (size_t)M * d.kv_dim * 4);
-    DM(pf.xba, (size_t)M * d.q_dim * 4); DM(pf.hb, (size_t)M * d.F * 4);
-    DM(pf.ws_m, slots * 4); DM(pf.ws_l, slots * 4); DM(pf.ws_acc, slots * d.hd * 4);
-    DM(pf.tickets, (size_t)M * d.KV * 4); CK(cudaMemset(pf.tickets, 0, (size_t)M * d.KV * 4));     // the merging CTA re-zeroes its ticket
-    if (d.exact) DM(pf.att, (size_t)M * d.H * d.max_seq * 4);
+    int r;
+    if ((r = alloc_layer_bufs(e, pf.buf, M))) return r;
     DM(pf.ids, (size_t)d.max_seq * 4);
     pf.M = M;
     return 0;
@@ -462,11 +493,11 @@ PrefillMvKern prefill_matvec_kernel(const Dims &d) {
     constexpr int RB = kPrefillRB;
     if (d.quant == 0x00u) return d.exact ? k_prefill_matvec_f32_exact<EPI> : k_prefill_matvec<0x00, EPI, RB, 8>;
     if (d.quant == 0x42u) return k_prefill_matvec<0x42, EPI, RB, 8>;
-    switch (d.gs) {
-        case 32: return k_prefill_matvec<0x80, EPI, RB, 2>;
-        case 64: return k_prefill_matvec<0x80, EPI, RB, 4>;
-        case 128: return k_prefill_matvec<0x80, EPI, RB, 8>;
-        case 256: return k_prefill_matvec<0x80, EPI, RB, 16>;
+    switch (matvec_lpg(d)) {
+        case 2: return k_prefill_matvec<0x80, EPI, RB, 2>;
+        case 4: return k_prefill_matvec<0x80, EPI, RB, 4>;
+        case 8: return k_prefill_matvec<0x80, EPI, RB, 8>;
+        case 16: return k_prefill_matvec<0x80, EPI, RB, 16>;
         default: return nullptr;
     }
 }
@@ -495,60 +526,38 @@ int run_prefill_matvec(nb200_engine *e, int epi, const Mat &mt, PrefillMvArgs a)
 int run_prefill_chunk(nb200_engine *e, uint32_t pos0, uint32_t m, const uint32_t *ids) {
     const Dims &d = e->d;
     auto &pf = e->pf;
+    const LayerBufs &b = pf.buf;
     const size_t kvl = (size_t)d.KV * d.max_seq * d.hd;
-    const uint32_t kvm = d.exact ? 0u : fast_attn_kvm(e);
+    const AttnChoice ac = pick_attn(e);
     int r;
     {
-        PrefillEmbedArgs a{e->emb.w, e->emb.aux, pf.x, ids, d};
+        PrefillEmbedArgs a{e->emb.w, e->emb.aux, b.x, ids, d};
         if ((r = launch<PrefillEmbedArgs>(e, k_prefill_embed, dim3(m), dim3(256), 0, a))) return r;
     }
     for (uint32_t l = 0; l < d.L; l++) {
         PrefillMvArgs a{};
         a.pos0 = pos0; a.m = m;
-        a.src = pf.x; a.src_stride = d.E; a.gain = e->norm_attn + (size_t)l * d.E;
-        a.out = pf.q; a.out_stride = d.q_dim; a.out_k = pf.kraw; a.k_stride = d.kv_dim; a.out_v = e->vc + l * kvl;
+        a.src = b.x; a.src_stride = d.E; a.gain = e->norm_attn + (size_t)l * d.E;
+        a.out = b.q; a.out_stride = d.q_dim; a.out_k = b.kraw; a.k_stride = d.kv_dim; a.out_v = e->vc + l * kvl;
         if ((r = run_prefill_matvec(e, EPI_QKV, e->qkv[l], a))) return r;
-
-        const float *knorm = e->knorm ? e->knorm + (size_t)l * d.hd : nullptr;
-        PrefillKrowArgs kr{pf.kraw, e->kc + l * kvl, knorm, e->rope_cos, e->rope_sin, pos0, kvm ? 1u : 0u, d};
-        if ((r = launch<PrefillKrowArgs>(e, k_prefill_krow, dim3(d.KV, m), dim3(32), 0, kr))) return r;
 
         PrefillAttnArgs pa{};
         pa.pos0 = pos0;
-        if (d.exact) {
-            AttnExactArgs &x = pa.ex;
-            x.q = pf.q; x.kraw = pf.kraw; x.kc = e->kc + l * kvl; x.vc = e->vc + l * kvl;
-            x.qnorm = e->qnorm ? e->qnorm + (size_t)l * d.hd : nullptr; x.knorm = knorm;
-            x.rope_cos = e->rope_cos; x.rope_sin = e->rope_sin; x.xba = pf.xba; x.att = pf.att; x.d = d;
-            pf.attn_kind = 1u;
-            if ((r = launch<PrefillAttnArgs>(e, k_prefill_attention_exact, dim3(d.H, m), dim3(kAttnThreads), 2 * d.hd * 4, pa))) return r;
-        } else {
-            AttnArgs &at = pa.at;
-            at.q = pf.q; at.kraw = pf.kraw; at.kc = e->kc + l * kvl; at.vc = e->vc + l * kvl;
-            at.qnorm = e->qnorm ? e->qnorm + (size_t)l * d.hd : nullptr; at.knorm = knorm;
-            at.rope_cos = e->rope_cos; at.rope_sin = e->rope_sin; at.xba = pf.xba;
-            at.ws_m = pf.ws_m; at.ws_l = pf.ws_l; at.ws_acc = pf.ws_acc; at.ticket = pf.tickets;
-            at.nsplit_max = e->nsplit_max; at.chunk_cap = e->chunk_cap; at.d = d;
-            void (*kern)(const PrefillAttnArgs) = k_prefill_attention;
-            switch (kvm) {
-                case 1: kern = k_prefill_attention_fast<1>; break;
-                case 2: kern = k_prefill_attention_fast<2>; break;
-                case 4: kern = k_prefill_attention_fast<4>; break;
-                case 8: kern = k_prefill_attention_fast<8>; break;
-                default: break;
-            }
-            const uint32_t smem = kvm ? attn_fast_smem_floats(d.kv_mul, d.hd, e->chunk_cap, e->nsplit_max, kWarps) * 4u : e->attn_smem;
-            pf.attn_kind = kvm ? (3u | (kvm << 8)) : 2u;
-            if ((r = launch<PrefillAttnArgs>(e, kern, dim3(e->nsplit_max, d.KV, m), dim3(kvm ? kThreads : kAttnThreads), smem, pa))) return r;
-        }
+        attn_args(e, b, l, pa.at, pa.ex);
+        PrefillKrowArgs kr{b.kraw, pa.at.kc, pa.at.knorm, e->rope_cos, e->rope_sin, pos0, ac.kvm ? 1u : 0u, d};
+        if ((r = launch<PrefillKrowArgs>(e, k_prefill_krow, dim3(d.KV, m), dim3(32), 0, kr))) return r;
+
+        pf.attn_kind = ac.kind;
+        const dim3 grid = d.exact ? dim3(d.H, m) : dim3(e->nsplit_max, d.KV, m);
+        if ((r = launch<PrefillAttnArgs>(e, ac.pf, grid, dim3(ac.threads), ac.smem, pa))) return r;
 
         a = PrefillMvArgs{};
         a.pos0 = pos0; a.m = m;
-        a.src = pf.xba; a.src_stride = d.q_dim; a.out = pf.x; a.out_stride = d.E;
+        a.src = b.xba; a.src_stride = d.q_dim; a.out = b.x; a.out_stride = d.E;
         if ((r = run_prefill_matvec(e, EPI_RESID, e->wo[l], a))) return r;
-        a.src = pf.x; a.src_stride = d.E; a.gain = e->norm_ffn + (size_t)l * d.E; a.out = pf.hb; a.out_stride = d.F;
+        a.src = b.x; a.src_stride = d.E; a.gain = e->norm_ffn + (size_t)l * d.E; a.out = b.hb; a.out_stride = d.F;
         if ((r = run_prefill_matvec(e, EPI_SWIGLU, e->w13[l], a))) return r;
-        a.src = pf.hb; a.src_stride = d.F; a.gain = nullptr; a.out = pf.x; a.out_stride = d.E;
+        a.src = b.hb; a.src_stride = d.F; a.gain = nullptr; a.out = b.x; a.out_stride = d.E;
         if ((r = run_prefill_matvec(e, EPI_RESID, e->w2[l], a))) return r;
     }
     return 0;
@@ -1051,15 +1060,13 @@ static int create_impl(nb200_engine **out, const uint8_t *img, uint64_t image_by
         e->tp_block_bytes = e->tp_off_hb + al(F * 8);      // {value, epoch} 64-bit elements
         DM(e->tp_block, e->tp_block_bytes);
         CK(cudaMemset(e->tp_block, 0, e->tp_block_bytes));
-        e->x = (float *)(e->tp_block + e->tp_off_x); e->xba = (float *)(e->tp_block + e->tp_off_xba); e->hb = (float *)(e->tp_block + e->tp_off_hb);
+        e->buf.x = (float *)(e->tp_block + e->tp_off_x); e->buf.xba = (float *)(e->tp_block + e->tp_off_xba); e->buf.hb = (float *)(e->tp_block + e->tp_off_hb);
         e->tp_peer[tp_rank] = e->tp_block;
-    } else {
-        DM(e->x, E * 4); DM(e->xba, QD * 4); DM(e->hb, F * 4);
     }
-    DM(e->q, QD * 4); DM(e->kraw, KD * 4); DM(e->logits, V * 4);
+    DM(e->logits, V * 4);
     DM(e->kc, kv_floats * 4); DM(e->vc, kv_floats * 4);
     CK(cudaMemset(e->kc, 0, kv_floats * 4)); CK(cudaMemset(e->vc, 0, kv_floats * 4));   // calloc'd in the reference (infer.c:47)
-    CK(cudaMemset(e->x, 0, E * 4)); CK(cudaMemset(e->logits, 0, V * 4));
+    CK(cudaMemset(e->logits, 0, V * 4));
     // Execution paths: the streaming kernel (stream.cuh) is the default in fast mode on one GPU; the CUDA-graph multi-kernel
     // path serves exact mode, tensor parallelism, LoRA and shapes the streaming kernel does not take.
     uint32_t nsm = (uint32_t)e->num_sms / e->g_KV;  // (kv head, split) items <= one per SM; same split in every path and TP size => identical bits
@@ -1073,9 +1080,8 @@ static int create_impl(nb200_engine **out, const uint8_t *img, uint64_t image_by
     uint32_t lpr = 1; while (lpr * 4 < d.hd) lpr <<= 1; if (lpr > 32) lpr = 32;
     const uint32_t rpw = 32 / lpr;
     e->attn_smem = (uint32_t)((d.kv_mul * d.hd + d.hd + cap + (size_t)kAttnWarps * rpw * d.hd) * 4);
-    DM(e->ws_m, (size_t)d.H * nsm * 4); DM(e->ws_l, (size_t)d.H * nsm * 4); DM(e->ws_acc, (size_t)d.H * nsm * d.hd * 4);
-    DM(e->tickets, d.KV * 4); CK(cudaMemset(e->tickets, 0, d.KV * 4));
-    if (d.exact) DM(e->att_exact, (size_t)d.H * d.max_seq * 4);
+    if ((r = alloc_layer_bufs(e, e->buf, 1))) return r;
+    CK(cudaMemset(e->buf.x, 0, E * 4));
     DM(e->ids_dev, ((size_t)d.max_seq + 8) * 4); CK(cudaMemset(e->ids_dev, 0, ((size_t)d.max_seq + 8) * 4));
     DM(e->seen, V); CK(cudaMemset(e->seen, 0, V));
     e->cls_grid = (uint32_t)e->num_sms * grid_mult();
@@ -1160,7 +1166,7 @@ static int calibrate_paths(nb200_engine *e) {
     const Dims &d = e->d;                                                                 // as created
     const size_t kv_floats = (size_t)d.L * d.KV * d.max_seq * d.hd;
     CK(cudaMemsetAsync(e->kc, 0, kv_floats * 4, e->stream)); CK(cudaMemsetAsync(e->vc, 0, kv_floats * 4, e->stream));
-    CK(cudaMemsetAsync(e->x, 0, (size_t)d.E * 4, e->stream)); CK(cudaMemsetAsync(e->logits, 0, (size_t)d.V * 4, e->stream));
+    CK(cudaMemsetAsync(e->buf.x, 0, (size_t)d.E * 4, e->stream)); CK(cudaMemsetAsync(e->logits, 0, (size_t)d.V * 4, e->stream));
     CK(cudaMemsetAsync(e->ids_dev, 0, ((size_t)d.max_seq + 8) * 4, e->stream));
     CK(cudaMemsetAsync(e->seen, 0, d.V, e->stream));
     e->seen_valid = false; e->seen_mirror.clear();
@@ -1479,10 +1485,10 @@ int nb200_read_buffer(nb200_engine *e, int field, uint32_t layer, uint32_t pos, 
     if (e->tp_size > 1 && (field == NB200_F_X || field == NB200_F_XBA || field == NB200_F_HB))
         return fail(NB200_EINVAL, "tensor-parallel engines keep x/xba/hb as {value, epoch} words; read them from a single-GPU engine");
     switch (field) {
-        case NB200_F_X: src = e->x; avail = d.E; break;
-        case NB200_F_XBA: src = e->xba; avail = d.q_dim; break;
-        case NB200_F_HB: src = e->hb; avail = d.F; break;
-        case NB200_F_Q: src = e->q; avail = d.q_dim; break;
+        case NB200_F_X: src = e->buf.x; avail = d.E; break;
+        case NB200_F_XBA: src = e->buf.xba; avail = d.q_dim; break;
+        case NB200_F_HB: src = e->buf.hb; avail = d.F; break;
+        case NB200_F_Q: src = e->buf.q; avail = d.q_dim; break;
         case NB200_F_LOGITS: src = e->logits; avail = d.V; break;
         case NB200_F_ACT_SCALE: src = e->dump_scales; avail = count; break;
         case NB200_F_ACT_I8: {
@@ -1508,7 +1514,7 @@ int nb200_write_x(nb200_engine *e, const float *x, uint32_t count) {
     if (e->tp_size > 1) return fail(NB200_EINVAL, "not available on tensor-parallel engines");
     CK(cudaSetDevice(e->device));
     CK(cudaStreamSynchronize(e->stream));
-    CK(cudaMemcpy(e->x, x, (size_t)count * 4, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(e->buf.x, x, (size_t)count * 4, cudaMemcpyHostToDevice));
     return 0;
 }
 
@@ -1644,7 +1650,7 @@ int op_matvec(uint32_t quant, float *out, const float *x, const void *w, size_t 
     int dev = 0, sms = 148;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if ((r = run_matvec(nullptr, EPI_STORE, m, a, false, sms))) return r;
+    if ((r = run_matvec(nullptr, EPI_STORE, m, a, sms))) return r;
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(out, dout.p, (size_t)d_rows * 4, cudaMemcpyDeviceToHost));
     return 0;

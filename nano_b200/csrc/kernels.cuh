@@ -138,14 +138,10 @@ struct MatvecArgs {
     uint32_t *ids;          // device copy of output_ids
     // debug dump of the prepared activation (written by CTA 0 when non-null)
     int8_t *dump_codes; float *dump_scales;
-    // persistent kernel: step state already in registers (saves an L2 round trip per phase)
-    uint32_t state_known, pos_val; float pen_val;
-    unsigned long long *dbg;     // optional: CTA 0 / thread 0 clock64() stamps inside the phase (tools/gpu_trace.py)
     Dims d;
     TpArgs tp;                   // tensor-parallel exchange (k_matvec<..., TP=true> only)
     const float *lora_add;       // RESID only: LoRA branch of the O projection, added to the matvec result BEFORE the residual (infer.c:898-908)
 };
-#define NB_STAMP(ptr, k) do { if ((ptr) && blockIdx.x == 0 && threadIdx.x == 0) (ptr)[k] = clock64(); } while (0)
 
 // ------------------------------------------------------------------------------------------------
 // small helpers
@@ -199,11 +195,10 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // Stage the fp32 source vector into shared memory with L2 (.cg) loads: the vector was produced by other
-// CTAs (another kernel, or another phase of the persistent kernel), so it must not come from L1 / the
-// non-coherent path.
+// CTAs (another kernel), so it must not come from L1 / the non-coherent path.
 // LL (tensor parallel): src is a vector of {value, epoch} words; spin per element until exchange tp->wait_ph has landed.
-// SB = loads in flight per thread: 1 keeps the register footprint of the persistent kernels, 4 (x float4) is what
-// the stand-alone matvec kernels use.
+// SB = loads in flight per thread: 1 (one float per load), or 4 (x float4), which the k_matvec and k_prefill_matvec
+// kernels use.
 template <int NT, bool LL = false, int SB = 1>
 __device__ __forceinline__ void stage_vector(const float *src, const float *__restrict__ gain, int n, float *stage, const TpArgs *tp = nullptr) {
     float *gstage = stage + n;                       // the rmsnorm gain rides along (one L2 latency, not two)
@@ -341,15 +336,12 @@ __device__ __forceinline__ int q80_code(float v, float sc, float rinv) {
 // tensor.c:21-46 (division and round-half-away exactly as the strict reference; zero group -> 0)
 template <int NT, bool LL = false, int SB = 1>
 __device__ void prep_q80(const float *src, const float *__restrict__ gain, int n, int gs, bool exact,
-                         unsigned char *act, float *stage, float *red, int8_t *dump_codes, float *dump_scales,
-                         unsigned long long *dbg = nullptr, const TpArgs *tp = nullptr) {
+                         unsigned char *act, float *stage, float *red, int8_t *dump_codes, float *dump_scales, const TpArgs *tp = nullptr) {
     int8_t *codes = reinterpret_cast<int8_t *>(act);
     float *scales = reinterpret_cast<float *>(act + ((n + 15) & ~15));
     stage_vector<NT, LL, SB>(src, gain, n, stage, tp);
-    NB_STAMP(dbg, 2);
     float inv = 1.0f;
     if (gain) inv = rms_inverse<NT>(stage, n, exact, red);
-    NB_STAMP(dbg, 3);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int G = n / gs, epl = gs / 32;      // elements per lane (gs in {32,64,128,256})
     for (int g = warp; g < G; g += NT / 32) {
@@ -729,8 +721,49 @@ __device__ __forceinline__ void rows_q4k(const uint8_t *__restrict__ W, const ui
 }
 
 // ------------------------------------------------------------------------------------------------
-// One fused matvec phase = activation prep -> row blocks -> epilogue, executed by `ncta` cooperating CTAs
-// (a whole kernel grid in the multi-kernel path, or the persistent grid of k_decode_mega).
+// Matvec epilogues: the arithmetic and destination of one finished row, shared by the token-path and prefill kernels
+// ------------------------------------------------------------------------------------------------
+// QKV: rows [0, q_dim) -> q, [q_dim, q_dim + kv_dim) -> raw k, the rest -> V-cache row `pos` of this layer ([KV][max_seq][hd])
+__device__ __forceinline__ void qkv_store(const Dims &d, uint32_t row, float v, float *q, float *kraw, float *vc, uint32_t pos) {
+    if (row < d.q_dim) q[row] = v;
+    else if (row < d.q_dim + d.kv_dim) kraw[row - d.q_dim] = v;
+    else {
+        const uint32_t c = row - d.q_dim - d.kv_dim, h = c / d.hd, i = c % d.hd;
+        vc[((size_t)h * d.max_seq + pos) * d.hd + i] = v;
+    }
+}
+// residual: x + v, with the LoRA term of the O projection (when non-null) added to v first (accum(xb2, o1) precedes x += xb2)
+__device__ __forceinline__ float resid_add(float x, float v, const float *lora_add, uint32_t row) {
+    if (lora_add) v = __fadd_rn(v, __ldcg(lora_add + row));
+    return __fadd_rn(x, v);
+}
+// SwiGLU of rows (2i, 2i+1) = (w1 row i, w3 row i); infer.c:937-944
+__device__ __forceinline__ float swiglu(float v1, float v3, bool exact) {
+    const float sg = __fdiv_rn(1.0f, __fadd_rn(1.0f, exact ? expf_ref(-v1) : expf(-v1)));
+    return __fmul_rn(__fmul_rn(v1, sg), v3);
+}
+
+// Exact-mode F32 (k_matvec_f32_exact, k_prefill_matvec_f32_exact): unit u = one row (a w1 / w3 row pair for SwiGLU) of one
+// position, the reference's left-to-right sum per row (infer.c:645-649), then the epilogue.
+template <int EPI>
+__device__ __forceinline__ void f32_exact_unit(const float *W, uint32_t n, uint32_t u, const float *x, const Dims &d, float *out,
+                                               float *out_k, float *out_v, uint32_t pos, const float *lora_add) {
+    constexpr int per = (EPI == EPI_SWIGLU) ? 2 : 1;
+    float res[2] = {0.0f, 0.0f};
+    for (int q = 0; q < per; q++) {
+        const float *wr = W + (size_t)(u * per + q) * n;
+        float acc = 0.0f;
+        for (uint32_t j = 0; j < n; j++) acc = __fadd_rn(acc, __fmul_rn(wr[j], x[j]));
+        res[q] = acc;
+    }
+    if (EPI == EPI_SWIGLU) out[u] = swiglu(res[0], res[1], true);
+    else if (EPI == EPI_STORE) out[u] = res[0];
+    else if (EPI == EPI_RESID) out[u] = resid_add(out[u], res[0], lora_add, u);
+    else if (EPI == EPI_QKV) qkv_store(d, u, res[0], out, out_k, out_v, pos);
+}
+
+// ------------------------------------------------------------------------------------------------
+// One fused matvec phase = activation prep -> row blocks -> epilogue, executed by the CTAs of one k_matvec grid.
 // ------------------------------------------------------------------------------------------------
 struct MatvecSmem {
     float red[32];
@@ -740,7 +773,7 @@ struct MatvecSmem {
 };
 
 // Weights never depend on activations: pull a warp's first row blocks of a matrix towards L2 ahead of time
-// (before the PDL wait / before a grid barrier), so the HBM latency hides behind the wait.
+// (before the PDL wait), so the HBM latency hides behind the wait.
 template <int QUANT, int RB>
 __device__ __forceinline__ void prefetch_row_blocks(const void *w, uint32_t rows, uint32_t n, uint32_t cta, uint32_t ncta, uint32_t max_iters,
                                                     const void *aux = nullptr, uint32_t aux_row_bytes = 0, const float *gain = nullptr) {
@@ -764,18 +797,18 @@ __device__ __forceinline__ void prefetch_row_blocks(const void *w, uint32_t rows
 // D (Q80 only) = weight tiles a warp keeps in flight along K: tile d+D of a row block is requested as soon as tile d has
 // been consumed, and the first D tiles are requested before the activation prologue.
 template <int QUANT, int EPI, int RB, int LPG, bool TP = false, int D = 1, int SB = 1>
-__device__ __forceinline__ void matvec_phase(const MatvecArgs &a, uint32_t cta, uint32_t ncta, unsigned char *act, MatvecSmem &ms) {
+__device__ __forceinline__ void matvec_phase(const MatvecArgs &a, unsigned char *act, MatvecSmem &ms) {
     const Dims &d = a.d;
+    const uint32_t cta = blockIdx.x;
     // tensor parallel: local row r is element rbase + r of the (replicated) output vector; QKV outputs stay local
     const uint32_t rbase = (TP && EPI != EPI_QKV) ? a.tp.row_base : 0u;
     const unsigned long long *out_ll = reinterpret_cast<const unsigned long long *>(a.out);     // TP: x is {value, epoch} words
     const bool exact = d.exact != 0;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t nblocks = (a.rows + RB - 1) / RB;
-    const uint32_t gwarp = cta * kWarps + warp, nwarps = ncta * kWarps;
+    const uint32_t gwarp = cta * kWarps + warp, nwarps = gridDim.x * kWarps;
     float *stage = reinterpret_cast<float *>(act + act_region_bytes(QUANT, a.n, (QUANT == 0x80) ? LPG * 16 : 1));
 
-    NB_STAMP(a.dbg, 0);
     // request this warp's first weight tile (and the residual it will add to) before the activation prologue
     Q80Tile<RB> pre[D];
     float xres[RB];
@@ -795,16 +828,15 @@ __device__ __forceinline__ void matvec_phase(const MatvecArgs &a, uint32_t cta, 
     }
 
     if (QUANT == 0x00) prep_f32<kThreads, TP, SB>(a.src, a.gain, a.n, exact, reinterpret_cast<float *>(act), stage, ms.red, &a.tp);
-    else if (QUANT == 0x80) { NB_STAMP(a.dbg, 1); prep_q80<kThreads, TP, SB>(a.src, a.gain, a.n, LPG * 16, exact, act, stage, ms.red, cta == 0 ? a.dump_codes : nullptr, a.dump_scales, a.dbg, &a.tp); }
+    else if (QUANT == 0x80) prep_q80<kThreads, TP, SB>(a.src, a.gain, a.n, LPG * 16, exact, act, stage, ms.red, cta == 0 ? a.dump_codes : nullptr, a.dump_scales, &a.tp);
     else prep_q4k<kThreads, TP, SB>(a.src, a.gain, a.n, exact, act, stage, ms.red, cta == 0 ? a.dump_codes : nullptr, a.dump_scales, &a.tp);
     uint32_t out_epoch = 0;
     if (TP && a.tp.signal_ph) out_epoch = tp_epoch(a.tp, a.tp.signal_ph);
 
-    NB_STAMP(a.dbg, 4);
-    const uint32_t pos = a.state_known ? a.pos_val : (a.st ? __ldcg(&a.st->pos) : 0);
+    const uint32_t pos = a.st ? __ldcg(&a.st->pos) : 0;
     float bestv = -FLT_MAX; uint32_t besti = 0xffffffffu;
     float pen = 1.0f;
-    if (EPI == EPI_CLS) pen = a.state_known ? a.pen_val : __ldcg(&a.st->penalty);
+    if (EPI == EPI_CLS) pen = __ldcg(&a.st->penalty);
 
     // One row block = dot products + epilogue.  `first` is a compile-time tag: the first block of a warp consumes the
     // tile (and residual) requested before the prologue straight from registers.  (A run-time `&pre : nullptr` select
@@ -847,14 +879,11 @@ __device__ __forceinline__ void matvec_phase(const MatvecArgs &a, uint32_t cta, 
         } else rows_q4k<RB>(static_cast<const uint8_t *>(a.w), static_cast<const uint8_t *>(a.w_aux), row0, a.rows, a.n, act, val);
 
         if (EPI == EPI_SWIGLU) {
-            // rows (2i, 2i+1) = (w1 row i, w3 row i); infer.c:937-944
 #pragma unroll
             for (int r = 0; r + 1 < RB; r += 2) {
                 const uint32_t row = row0 + r;
                 if (lane == 0 && row + 1 < a.rows) {
-                    const float v1 = val[r], v3 = val[r + 1];
-                    const float sg = __fdiv_rn(1.0f, __fadd_rn(1.0f, exact ? expf_ref(-v1) : expf(-v1)));
-                    const float hv = __fmul_rn(__fmul_rn(v1, sg), v3);
+                    const float hv = swiglu(val[r], val[r + 1], exact);
                     if (TP) tp_store(a.tp, rbase + (row >> 1), hv, out_epoch); else a.out[row >> 1] = hv;
                 }
             }
@@ -868,20 +897,12 @@ __device__ __forceinline__ void matvec_phase(const MatvecArgs &a, uint32_t cta, 
                 else if (EPI == EPI_RESID) {
                     if (lane == 0) {
                         const float xo = kFirst ? xres[r] : (TP ? __uint_as_float((uint32_t)__ldcg(out_ll + rbase + row)) : __ldcg(a.out + rbase + row));
-                        if (a.lora_add) v = __fadd_rn(v, __ldcg(a.lora_add + rbase + row));       // accum(xb2, o1) precedes x += xb2
-                        const float xn = __fadd_rn(xo, v);
+                        const float xn = resid_add(xo, v, a.lora_add, rbase + row);
                         if (TP) tp_store(a.tp, rbase + row, xn, out_epoch); else a.out[row] = xn;
                     }
                 }
                 else if (EPI == EPI_QKV) {
-                    if (lane == 0) {
-                        if (row < d.q_dim) a.out[row] = v;
-                        else if (row < d.q_dim + d.kv_dim) a.out_k[row - d.q_dim] = v;
-                        else {
-                            const uint32_t c = row - d.q_dim - d.kv_dim, h = c / d.hd, i = c % d.hd;
-                            a.out_v[((size_t)h * d.max_seq + pos) * d.hd + i] = v;
-                        }
-                    }
+                    if (lane == 0) qkv_store(d, row, v, a.out, a.out_k, a.out_v, pos);
                 } else if (EPI == EPI_CLS) {
                     // infer.c:1156-1167 penalty (division, any sign), then first-max argmax :1026-1037
                     if (pen != 1.0f && __ldcg(a.seen + rbase + row)) v = __fdiv_rn(v, pen);      // x / 1.0f == x: skip the lookup
@@ -896,7 +917,6 @@ __device__ __forceinline__ void matvec_phase(const MatvecArgs &a, uint32_t cta, 
         for (uint32_t rb = gwarp + nwarps; rb < nblocks; rb += nwarps) do_block(rb, std::false_type{});
     }
 
-    NB_STAMP(a.dbg, 5);
     if (EPI == EPI_CLS) {
         // rows were visited in ascending order per warp, so (bestv,besti) already holds the warp's first max
         if (lane == 0) { ms.best_v[warp] = bestv; ms.best_i[warp] = besti; }
@@ -909,6 +929,22 @@ __device__ __forceinline__ void matvec_phase(const MatvecArgs &a, uint32_t cta, 
         }
         __syncthreads();
     }
+}
+
+// End of a step, by one thread, given the step's argmax bi: mark the consumed id seen, append bi (or take the forced prompt
+// id), advance pos, publish the token the next step consumes and return it.
+__device__ __forceinline__ uint32_t finish_step(DevState *st, uint32_t *ids, uint8_t *seen_rw, uint32_t bi) {
+    if (bi == 0xffffffffu) bi = 0;     // all-NaN row: the reference's argmax returns index 0
+    const uint32_t p = __ldcg(&st->pos);
+    uint32_t nxt = bi;
+    if (__ldcg(&st->advance)) {
+        seen_rw[__ldcg(ids + p)] = 1;                           // ids[0..p] are "seen" for step p+1
+        const bool forced = (p + 1 < __ldcg(&st->n_prompt));   // infer.c:1250 is_prefilling
+        if (!forced) ids[p + 1] = bi; else nxt = __ldcg(ids + p + 1);
+        st->pos = p + 1;
+    }
+    st->next_token = nxt;
+    return nxt;
 }
 
 // Final argmax over the per-CTA partials + state update, by ONE full CTA.  Returns (in every thread) the token
@@ -949,20 +985,8 @@ __device__ __forceinline__ uint32_t cls_finalize(const MatvecArgs &a, uint32_t n
             }
             h->epoch_base = epoch;
         }
-        if (bi == 0xffffffffu) bi = 0;     // all-NaN row: the reference's argmax returns index 0
-        DevState *st = a.st_rw;
-        st->cls_ticket = 0;
-        const uint32_t p = __ldcg(&st->pos);
-        uint32_t nxt = bi;
-        if (__ldcg(&st->advance)) {
-            const uint32_t tok_in = __ldcg(a.ids + p);
-            a.seen_rw[tok_in] = 1;                                  // ids[0..p] are "seen" for step p+1
-            const bool forced = (p + 1 < __ldcg(&st->n_prompt));   // infer.c:1250 is_prefilling
-            if (!forced) a.ids[p + 1] = bi; else nxt = __ldcg(a.ids + p + 1);
-            st->pos = p + 1;
-        }
-        st->next_token = nxt;
-        ms.flag = nxt;
+        a.st_rw->cls_ticket = 0;
+        ms.flag = finish_step(a.st_rw, a.ids, a.seen_rw, bi);
     }
     __syncthreads();
     return ms.flag;
@@ -976,7 +1000,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_matvec(const MatvecArgs a) {
     pdl_launch_dependents();
     prefetch_row_blocks<QUANT, RB>(a.w, a.rows, a.n, blockIdx.x, gridDim.x, 4);
     pdl_wait();
-    matvec_phase<QUANT, EPI, RB, LPG, TP, D, 4>(a, blockIdx.x, gridDim.x, act, ms);
+    matvec_phase<QUANT, EPI, RB, LPG, TP, D, 4>(a, act, ms);
 
     if (EPI == EPI_CLS) {
         if (threadIdx.x == 0) {
@@ -1000,34 +1024,10 @@ __global__ void __launch_bounds__(256) k_matvec_f32_exact(const MatvecArgs a) {
     pdl_wait();
     prep_f32<256>(a.src, a.gain, a.n, true, reinterpret_cast<float *>(act), reinterpret_cast<float *>(act) + a.n, red);   // smem: 3n floats
     const float *x = reinterpret_cast<const float *>(act);
-    const float *W = static_cast<const float *>(a.w);
-    const Dims &d = a.d;
     const uint32_t pos = a.st ? a.st->pos : 0;
     const uint32_t nunits = (EPI == EPI_SWIGLU) ? a.rows / 2 : a.rows;
-    for (uint32_t u = blockIdx.x * 256 + threadIdx.x; u < nunits; u += gridDim.x * 256) {
-        const int per = (EPI == EPI_SWIGLU) ? 2 : 1;
-        float res[2] = {0.0f, 0.0f};
-        for (int p = 0; p < per; p++) {
-            const float *wr = W + (size_t)(u * per + p) * a.n;
-            float acc = 0.0f;
-            for (uint32_t j = 0; j < a.n; j++) acc = __fadd_rn(acc, __fmul_rn(wr[j], x[j]));
-            res[p] = acc;
-        }
-        const uint32_t row = u;
-        if (EPI == EPI_SWIGLU) {
-            const float sg = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf_ref(-res[0])));
-            a.out[row] = __fmul_rn(__fmul_rn(res[0], sg), res[1]);
-        } else if (EPI == EPI_STORE) a.out[row] = res[0];
-        else if (EPI == EPI_RESID) a.out[row] = __fadd_rn(a.out[row], a.lora_add ? __fadd_rn(res[0], a.lora_add[row]) : res[0]);
-        else if (EPI == EPI_QKV) {
-            if (row < d.q_dim) a.out[row] = res[0];
-            else if (row < d.q_dim + d.kv_dim) a.out_k[row - d.q_dim] = res[0];
-            else {
-                const uint32_t c = row - d.q_dim - d.kv_dim, h = c / d.hd, i = c % d.hd;
-                a.out_v[((size_t)h * d.max_seq + pos) * d.hd + i] = res[0];
-            }
-        }
-    }
+    for (uint32_t u = blockIdx.x * 256 + threadIdx.x; u < nunits; u += gridDim.x * 256)
+        f32_exact_unit<EPI>(static_cast<const float *>(a.w), a.n, u, x, a.d, a.out, a.out_k, a.out_v, pos, a.lora_add);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1103,32 +1103,39 @@ struct EmbedArgs {
     uint32_t ll;                        // tensor parallel: x is a vector of {value, epoch} words (epoch unused for the local embedding)
 };
 
-NB_K __global__ void __launch_bounds__(256) k_embed(const EmbedArgs a) {
-    pdl_launch_dependents();
-    pdl_wait();
-    const Dims &d = a.d;
-    const uint32_t tok = a.st->use_token ? a.st->token : a.ids[a.st->pos];
+// one embedding row -> x, by one CTA (k_embed, k_prefill_embed, the streaming kernel); LL: x as for EmbedArgs::ll
+template <int NT, bool LL = false>
+__device__ __forceinline__ void embed_row(const void *w, const void *aux, float *x, uint32_t tok, const Dims &d) {
     const uint32_t E = d.E;
-    for (uint32_t i = threadIdx.x; i < E; i += 256) {
+    for (uint32_t i = threadIdx.x; i < E; i += NT) {
         float v;
-        if (d.quant == 0x00u) v = static_cast<const float *>(a.w)[(size_t)tok * E + i];
+        if (d.quant == 0x00u) v = __ldg(static_cast<const float *>(w) + (size_t)tok * E + i);
         else if (d.quant == 0x80u) {
-            const int8_t c = static_cast<const int8_t *>(a.w)[(size_t)tok * E + i];
-            const float s = static_cast<const float *>(a.w_aux)[((size_t)tok * E + i) / d.gs];
+            const int8_t c = __ldg(static_cast<const int8_t *>(w) + (size_t)tok * E + i);
+            const float s = __ldg(static_cast<const float *>(aux) + ((size_t)tok * E + i) / d.gs);
             v = __fmul_rn((float)c, s);                                  // tensor.c:15-19
         } else {
             const uint32_t bpr = E / 256, blk = i >> 8, e = i & 255, g = e >> 5, j = g & 3;
-            const uint8_t byte = static_cast<const uint8_t *>(a.w)[(size_t)tok * (E / 2) + (i >> 1)];
+            const uint8_t byte = __ldg(static_cast<const uint8_t *>(w) + (size_t)tok * (E / 2) + (i >> 1));
             const uint32_t c = (i & 1) ? (byte >> 4) : (byte & 0x0f);
-            const uint32_t *rec = reinterpret_cast<const uint32_t *>(static_cast<const uint8_t *>(a.w_aux) + ((size_t)tok * bpr + blk) * 20);
-            const float ss = __uint_as_float(rec[0]), sbi = __uint_as_float(rec[1]);
-            const uint32_t bs = (rec[2] >> (8 * j)) & 0xff, bb = (rec[3] >> (8 * j)) & 0xff, bh = (rec[4] >> (8 * j)) & 0xff;
+            const uint32_t *rec = reinterpret_cast<const uint32_t *>(static_cast<const uint8_t *>(aux) + ((size_t)tok * bpr + blk) * 20);
+            const float ss = __uint_as_float(__ldg(rec)), sbi = __uint_as_float(__ldg(rec + 1));
+            const uint32_t bs = (__ldg(rec + 2) >> (8 * j)) & 0xff, bb = (__ldg(rec + 3) >> (8 * j)) & 0xff, bh = (__ldg(rec + 4) >> (8 * j)) & 0xff;
             const uint32_t s6 = (g < 4) ? (bs & 0x3f) : ((((bs >> 6) << 4) | (bh & 0x0f)) & 0x3f);
             const uint32_t b6 = (g < 4) ? (bb & 0x3f) : ((((bb >> 6) << 4) | (bh >> 4)) & 0x3f);
             v = __fsub_rn(__fmul_rn((float)c, __fmul_rn((float)s6, ss)), __fmul_rn((float)b6, sbi));   // tensor.c:274
         }
-        if (a.ll) reinterpret_cast<unsigned long long *>(a.x)[i] = tp_pack(__float_as_uint(v), 0); else a.x[i] = v;
+        if constexpr (LL) reinterpret_cast<unsigned long long *>(x)[i] = tp_pack(__float_as_uint(v), 0);
+        else x[i] = v;
     }
+}
+
+NB_K __global__ void __launch_bounds__(256) k_embed(const EmbedArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const uint32_t tok = a.st->use_token ? a.st->token : a.ids[a.st->pos];
+    if (a.ll) embed_row<256, true>(a.w, a.w_aux, a.x, tok, a.d);
+    else embed_row<256>(a.w, a.w_aux, a.x, tok, a.d);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1420,6 +1427,14 @@ __device__ __forceinline__ void attn_stream_partial(const Dims &d, const float *
 #undef AT_STAMP
 }
 
+// Split-KV plan of a position attending to rows [0, range) (k_attention_fast, k_attention and their prefill variants): chunk
+// rows per split, at least 32 and a multiple of 8, at most chunk_cap; nsplit <= nsplit_max splits.
+__device__ __forceinline__ void attn_split_plan(uint32_t range, uint32_t nsplit_max, uint32_t chunk_cap, uint32_t &chunk, uint32_t &nsplit) {
+    chunk = max((range + nsplit_max - 1) / nsplit_max, 32u);
+    chunk = min((chunk + 7u) & ~7u, chunk_cap);
+    nsplit = (range + chunk - 1) / chunk;
+}
+
 // One (kv head, split) item of the grid-wide paths: partial -> HBM workspace; the last CTA of the kv head merges.
 // smem (floats): streaming workspace | wsc[KVM*nsplit_max] | stat[2*KVM]
 template <int KVM, int NT, bool TP = false>
@@ -1521,7 +1536,7 @@ __device__ __forceinline__ void attn_item(const AttnArgs &a, uint32_t g, uint32_
 }
 
 template <int KVM, bool TP = false>
-__global__ void __launch_bounds__(kThreads) k_attention_fast(const AttnArgs a) {      // same CTA shape as the megakernel => same bits
+__global__ void __launch_bounds__(kThreads) k_attention_fast(const AttnArgs a) {
     extern __shared__ __align__(16) float sm[];
     __shared__ uint32_t is_last;
     pdl_launch_dependents();
@@ -1531,10 +1546,8 @@ __global__ void __launch_bounds__(kThreads) k_attention_fast(const AttnArgs a) {
     const uint32_t pos = __ldcg(&a.st->pos);
     const uint32_t range = __ldcg(&a.st->is_causal) ? pos + 1 : d.max_seq;
     AG_STAMP(blockIdx.x == 0 && blockIdx.y == 0, 1);
-    uint32_t chunk = (range + a.nsplit_max - 1) / a.nsplit_max;
-    chunk = max(chunk, 32u);
-    chunk = min((chunk + 7u) & ~7u, a.chunk_cap);
-    const uint32_t nsplit = (range + chunk - 1) / chunk;
+    uint32_t chunk, nsplit;
+    attn_split_plan(range, a.nsplit_max, a.chunk_cap, chunk, nsplit);
     if (blockIdx.x >= nsplit) return;
     attn_item<KVM, kThreads, TP>(a, blockIdx.y, blockIdx.x, pos, range, chunk, nsplit, sm, is_last);
 }
@@ -1546,10 +1559,8 @@ __device__ __forceinline__ void attn_generic_cta(const AttnArgs &a, uint32_t g, 
     const Dims &d = a.d;
     const bool exact = d.exact != 0;
     const uint32_t hd = d.hd, kvm = d.kv_mul;
-    uint32_t chunk = (range + a.nsplit_max - 1) / a.nsplit_max;
-    chunk = max(chunk, 32u);
-    chunk = min((chunk + 7u) & ~7u, a.chunk_cap);
-    const uint32_t nsplit = (range + chunk - 1) / chunk;
+    uint32_t chunk, nsplit;
+    attn_split_plan(range, a.nsplit_max, a.chunk_cap, chunk, nsplit);
     if (split >= nsplit) return;
     const uint32_t t0 = split * chunk, t1 = min(range, t0 + chunk), len = t1 - t0;
     const bool owner = (pos >= t0 && pos < t1);
@@ -1754,13 +1765,12 @@ NB_K __global__ void __launch_bounds__(kAttnThreads) k_attention_exact(const Att
 struct FinalizeArgs { float *logits; uint32_t V; const uint8_t *seen; uint8_t *seen_rw; uint32_t *ids; DevState *st; };
 
 NB_K __global__ void __launch_bounds__(1024) k_cls_finalize(const FinalizeArgs a) {
-    float *logits = a.logits; const uint32_t V = a.V; const uint8_t *seen = a.seen; uint8_t *seen_rw = a.seen_rw;
-    uint32_t *ids = a.ids; DevState *st = a.st;
+    float *logits = a.logits; const uint32_t V = a.V; const uint8_t *seen = a.seen;
     __shared__ float bvs[32];
     __shared__ uint32_t bis[32];
     pdl_launch_dependents();
     pdl_wait();
-    const float pen = st->penalty;
+    const float pen = a.st->penalty;
     float bv = -FLT_MAX; uint32_t bi = 0xffffffffu;
     for (uint32_t i = threadIdx.x; i < V; i += 1024) {
         float v = logits[i];
@@ -1775,16 +1785,7 @@ NB_K __global__ void __launch_bounds__(1024) k_cls_finalize(const FinalizeArgs a
     __syncthreads();
     if (threadIdx.x == 0) {
         for (int w = 1; w < 32; w++) if (bvs[w] > bv || (bvs[w] == bv && bis[w] < bi)) { bv = bvs[w]; bi = bis[w]; }
-        if (bi == 0xffffffffu) bi = 0;
-        const uint32_t p = st->pos;
-        if (st->advance) {
-            const uint32_t tok_in = ids[p];
-            seen_rw[tok_in] = 1;
-            const bool forced = (p + 1 < st->n_prompt);
-            if (!forced) ids[p + 1] = bi;
-            st->next_token = forced ? ids[p + 1] : bi;
-            st->pos = p + 1;
-        } else st->next_token = bi;
+        finish_step(a.st, a.ids, a.seen_rw, bi);
     }
 }
 
@@ -1811,32 +1812,6 @@ __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
     unsigned int v;
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
-}
-
-// embedding row -> x (infer.c:987-988 + load-time dequantisation), by one CTA
-template <int NT>
-__device__ __forceinline__ void embed_row(const void *w, const void *aux, float *x, uint32_t tok, const Dims &d) {
-    const uint32_t E = d.E;
-    for (uint32_t i = threadIdx.x; i < E; i += NT) {
-        float v;
-        if (d.quant == 0x00u) v = __ldg(static_cast<const float *>(w) + (size_t)tok * E + i);
-        else if (d.quant == 0x80u) {
-            const int8_t c = __ldg(static_cast<const int8_t *>(w) + (size_t)tok * E + i);
-            const float s = __ldg(static_cast<const float *>(aux) + ((size_t)tok * E + i) / d.gs);
-            v = __fmul_rn((float)c, s);                                  // tensor.c:15-19
-        } else {
-            const uint32_t bpr = E / 256, blk = i >> 8, e = i & 255, g = e >> 5, j = g & 3;
-            const uint8_t byte = __ldg(static_cast<const uint8_t *>(w) + (size_t)tok * (E / 2) + (i >> 1));
-            const uint32_t c = (i & 1) ? (byte >> 4) : (byte & 0x0f);
-            const uint32_t *rec = reinterpret_cast<const uint32_t *>(static_cast<const uint8_t *>(aux) + ((size_t)tok * bpr + blk) * 20);
-            const float ss = __uint_as_float(__ldg(rec)), sbi = __uint_as_float(__ldg(rec + 1));
-            const uint32_t bs = (__ldg(rec + 2) >> (8 * j)) & 0xff, bb = (__ldg(rec + 3) >> (8 * j)) & 0xff, bh = (__ldg(rec + 4) >> (8 * j)) & 0xff;
-            const uint32_t s6 = (g < 4) ? (bs & 0x3f) : ((((bs >> 6) << 4) | (bh & 0x0f)) & 0x3f);
-            const uint32_t b6 = (g < 4) ? (bb & 0x3f) : ((((bb >> 6) << 4) | (bh >> 4)) & 0x3f);
-            v = __fsub_rn(__fmul_rn((float)c, __fmul_rn((float)s6, ss)), __fmul_rn((float)b6, sbi));   // tensor.c:274
-        }
-        x[i] = v;
-    }
 }
 
 }  // namespace nb

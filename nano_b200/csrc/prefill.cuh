@@ -37,35 +37,22 @@ struct PrefillMvArgs {
     Dims d;
 };
 
-// matvec_phase's epilogues (kernels.cuh) for one position of the chunk: lane 0 stores
+// the matvec epilogues (kernels.cuh) for one position of the chunk: lane 0 stores
 template <int EPI, int RB>
 __device__ __forceinline__ void prefill_store(const PrefillMvArgs &a, uint32_t p, uint32_t row0, const float (&val)[RB]) {
     if ((threadIdx.x & 31) != 0) return;
-    const Dims &d = a.d;
     float *out = a.out + (size_t)p * a.out_stride;
     if (EPI == EPI_SWIGLU) {
 #pragma unroll
-        for (int r = 0; r + 1 < RB; r += 2) {
-            const uint32_t row = row0 + r;
-            if (row + 1 < a.rows) {
-                const float v1 = val[r], v3 = val[r + 1];
-                const float sg = __fdiv_rn(1.0f, __fadd_rn(1.0f, d.exact ? expf_ref(-v1) : expf(-v1)));
-                out[row >> 1] = __fmul_rn(__fmul_rn(v1, sg), v3);
-            }
-        }
+        for (int r = 0; r + 1 < RB; r += 2)
+            if (row0 + r + 1 < a.rows) out[(row0 + r) >> 1] = swiglu(val[r], val[r + 1], a.d.exact != 0);
     } else {
 #pragma unroll
         for (int r = 0; r < RB; r++) {
             const uint32_t row = row0 + r;
             if (row >= a.rows) break;
-            const float v = val[r];
-            if (EPI == EPI_RESID) out[row] = __fadd_rn(__ldcg(out + row), v);
-            else if (row < d.q_dim) out[row] = v;                                          // EPI_QKV
-            else if (row < d.q_dim + d.kv_dim) a.out_k[(size_t)p * a.k_stride + row - d.q_dim] = v;
-            else {
-                const uint32_t c = row - d.q_dim - d.kv_dim, h = c / d.hd, i = c % d.hd;
-                a.out_v[((size_t)h * d.max_seq + a.pos0 + p) * d.hd + i] = v;
-            }
+            if (EPI == EPI_RESID) out[row] = resid_add(__ldcg(out + row), val[r], nullptr, row);
+            else qkv_store(a.d, row, val[r], out, a.out_k + (size_t)p * a.k_stride, a.out_v, a.pos0 + p);
         }
     }
 }
@@ -157,7 +144,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_prefill_matvec(const PrefillMvA
     }
 }
 
-// exact-mode F32 (k_matvec_f32_exact over the chunk): one thread per row, the reference's left-to-right sum per position
+// exact-mode F32 (k_matvec_f32_exact over the chunk): one thread per unit, f32_exact_unit per position
 template <int EPI>
 __global__ void __launch_bounds__(kThreads, 1) k_prefill_matvec_f32_exact(const PrefillMvArgs a) {
     extern __shared__ __align__(16) unsigned char act[];
@@ -168,37 +155,14 @@ __global__ void __launch_bounds__(kThreads, 1) k_prefill_matvec_f32_exact(const 
     float *stage = reinterpret_cast<float *>(act + (size_t)a.m * a.act_bytes);
     for (uint32_t p = 0; p < a.m; p++)
         prep_f32<kThreads>(a.src + (size_t)p * a.src_stride, a.gain, n, true, reinterpret_cast<float *>(act + (size_t)p * a.act_bytes), stage, red);
-    const Dims &d = a.d;
-    const float *W = static_cast<const float *>(a.w);
     const uint32_t nunits = (EPI == EPI_SWIGLU) ? a.rows / 2 : a.rows;
-    constexpr int per = (EPI == EPI_SWIGLU) ? 2 : 1;
-    for (uint32_t u = blockIdx.x * kThreads + threadIdx.x; u < nunits; u += gridDim.x * kThreads) {
-        for (uint32_t p = 0; p < a.m; p++) {
-            const float *x = reinterpret_cast<const float *>(act + (size_t)p * a.act_bytes);
-            float res[2] = {0.0f, 0.0f};
-            for (int q = 0; q < per; q++) {
-                const float *wr = W + (size_t)(u * per + q) * n;
-                float acc = 0.0f;
-                for (uint32_t j = 0; j < n; j++) acc = __fadd_rn(acc, __fmul_rn(wr[j], x[j]));
-                res[q] = acc;
-            }
-            float *out = a.out + (size_t)p * a.out_stride;
-            const uint32_t row = u;
-            if (EPI == EPI_SWIGLU) {
-                const float sg = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf_ref(-res[0])));
-                out[row] = __fmul_rn(__fmul_rn(res[0], sg), res[1]);
-            } else if (EPI == EPI_RESID) out[row] = __fadd_rn(out[row], res[0]);
-            else if (row < d.q_dim) out[row] = res[0];                                      // EPI_QKV
-            else if (row < d.q_dim + d.kv_dim) a.out_k[(size_t)p * a.k_stride + row - d.q_dim] = res[0];
-            else {
-                const uint32_t c = row - d.q_dim - d.kv_dim, h = c / d.hd, i = c % d.hd;
-                a.out_v[((size_t)h * d.max_seq + a.pos0 + p) * d.hd + i] = res[0];
-            }
-        }
-    }
+    for (uint32_t u = blockIdx.x * kThreads + threadIdx.x; u < nunits; u += gridDim.x * kThreads)
+        for (uint32_t p = 0; p < a.m; p++)
+            f32_exact_unit<EPI>(static_cast<const float *>(a.w), n, u, reinterpret_cast<const float *>(act + (size_t)p * a.act_bytes), a.d,
+                                a.out + (size_t)p * a.out_stride, a.out_k + (size_t)p * a.k_stride, a.out_v, a.pos0 + p, nullptr);
 }
 
-// the embedding rows of the chunk's ids (k_embed's lookup and dequantisation), one CTA per position
+// the embedding rows of the chunk's ids (embed_row, as k_embed), one CTA per position
 struct PrefillEmbedArgs { const void *w, *w_aux; float *x; const uint32_t *ids; Dims d; };
 NB_K __global__ void __launch_bounds__(256) k_prefill_embed(const PrefillEmbedArgs a) {
     pdl_launch_dependents();
@@ -261,13 +225,6 @@ __device__ __forceinline__ AttnArgs prefill_attn_at(const PrefillAttnArgs &pa, u
     a.ws_m += p * slots; a.ws_l += p * slots; a.ws_acc += p * slots * d.hd; a.ticket += (size_t)p * d.KV;
     return a;
 }
-// k_attention_fast / k_attention's split count for a causal position
-__device__ __forceinline__ uint32_t prefill_attn_chunk(const AttnArgs &a, uint32_t range) {
-    uint32_t chunk = (range + a.nsplit_max - 1) / a.nsplit_max;
-    chunk = max(chunk, 32u);
-    return min((chunk + 7u) & ~7u, a.chunk_cap);
-}
-
 template <int KVM>
 __global__ void __launch_bounds__(kThreads, 1) k_prefill_attention_fast(const PrefillAttnArgs pa) {
     extern __shared__ __align__(16) float sm[];
@@ -276,7 +233,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_prefill_attention_fast(const Pr
     pdl_wait();
     const uint32_t p = blockIdx.z, pos = pa.pos0 + p, range = pos + 1;
     const AttnArgs a = prefill_attn_at(pa, p);
-    const uint32_t chunk = prefill_attn_chunk(a, range), nsplit = (range + chunk - 1) / chunk;
+    uint32_t chunk, nsplit;
+    attn_split_plan(range, a.nsplit_max, a.chunk_cap, chunk, nsplit);
     if (blockIdx.x >= nsplit) return;
     attn_item<KVM, kThreads, false>(a, blockIdx.y, blockIdx.x, pos, range, chunk, nsplit, sm, is_last);
 }
