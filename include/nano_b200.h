@@ -169,6 +169,37 @@ int nb200_decode_greedy(nb200_engine *e, uint32_t *ids, uint32_t n_prompt, uint3
  * so their fast-mode K/V bits do not change), tensor cores, non-causal (seq2seq) attention. */
 int nb200_prefill(nb200_engine *e, const uint32_t *ids, uint32_t pos0, uint32_t n, float *device_ms);
 
+/* Batched multi-session decode (no reference counterpart).  A batch is attached to an engine and shares its weights; it holds
+ * n_slots sessions ("slots"), each with its own K / V cache (laid out like the engine's and zeroed at creation, n_kv_head *
+ * head_dim * max_seq_len * n_layer * 8 bytes), repetition-penalty seen set and logits row.  n_slots is not capped at the pass size.
+ *   nb200_batch_prefill      nb200_prefill into one slot's cache.
+ *   nb200_batch_next_greedy  entry i does what nb200_next_greedy(e, ids[i], pos[i], 0, repetition_penalty[i], &next_tokens[i])
+ *                            does, in slot slots[i]: it consumes ids[i][pos[i]] at pos[i], ids[i][0..pos[i]) feed the penalty (a
+ *                            rewind or a new session in a slot resets its seen set, as for the engine), and the slot's logits end
+ *                            up as nb200_read_logits returns them after that call (penalised).  The entries run in passes of up
+ *                            to M (info[0], at most 16) positions per pass over the weights.  device_ms (optional): CUDA-event
+ *                            time of the call.
+ *   nb200_batch_read_logits / nb200_batch_read_kv  a slot's logits row, and its K / V cache rows as nb200_read_buffer gives them.
+ *   nb200_batch_info         [0] M, [1] n_slots, [2] the attention kernel (encoded as nb200_config.reserved[4]), [3] 0.
+ * A batch always runs the multi-kernel path's arithmetic, and a row's value depends neither on the other entries of its pass nor
+ * on how many there are: each slot's ids, logits and K / V rows are bit-identical to those of an engine created with the same
+ * flags plus NB200_FLAG_NO_STREAM running that session alone (nb200_prefill + nb200_next_greedy) -- also when the batch's own
+ * engine runs the streaming kernel -- and in exact mode to the strict reference.  The engine's own cache, logits, seen set,
+ * results and nb200_config.reserved[3..6] are not changed by a batch; its calls share the engine's stream.
+ * NB200_EINVAL, with nothing written: a tensor-parallel engine or an active LoRA plug-in (checked at every call), n_slots == 0,
+ * n == 0, a slot >= n_slots or the same slot twice in one call, a position >= min(max_seq_len, block_size), an id >= vocab_size.
+ * Destroy every batch before its engine.  Not covered: temperature sampling, non-causal attention, LoRA, tensor parallelism. */
+typedef struct nb200_batch nb200_batch;
+int nb200_batch_create(nb200_engine *e, uint32_t n_slots, nb200_batch **out);
+void nb200_batch_destroy(nb200_batch *b);
+int nb200_batch_prefill(nb200_batch *b, uint32_t slot, const uint32_t *ids, uint32_t pos0, uint32_t n, float *device_ms);
+int nb200_batch_next_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t *const *ids, const uint32_t *pos,
+                            const float *repetition_penalty, uint32_t *next_tokens, float *device_ms);
+int nb200_batch_read_logits(nb200_batch *b, uint32_t slot, float *host_logits);
+int nb200_batch_read_kv(nb200_batch *b, uint32_t slot, int field /* NB200_F_KROW | NB200_F_VROW */, uint32_t layer, uint32_t pos,
+                        float *dst, uint32_t count);
+int nb200_batch_info(const nb200_batch *b, uint32_t info[4]);
+
 /* introspection for parity tests */
 int nb200_read_buffer(nb200_engine *e, int field, uint32_t layer, uint32_t pos, float *dst, uint32_t count);
 int nb200_write_x(nb200_engine *e, const float *x, uint32_t count);

@@ -33,7 +33,7 @@ def _newer(target: str, sources) -> bool:
 
 # translation units of libnano_b200.so and what each depends on (besides itself)
 UNITS = {
-    "engine.cu": ["kernels.cuh", "prefill.cuh", "expf_ref.cuh", "stream_args.h", "stream_host.h", "sample_host.h", "../../include/nano_b200.h"],
+    "engine.cu": ["kernels.cuh", "prefill.cuh", "batch.cuh", "expf_ref.cuh", "stream_args.h", "stream_host.h", "sample_host.h", "../../include/nano_b200.h"],
     "stream.cu": ["kernels.cuh", "expf_ref.cuh", "stream_args.h", "stream_host.h", "stream.cuh"],
     "sample.cu": ["kernels.cuh", "expf_ref.cuh", "sample_host.h"],
 }

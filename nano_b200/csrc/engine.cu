@@ -27,7 +27,7 @@
 
 #include "../../include/nano_b200.h"
 #include "kernels.cuh"
-#include "prefill.cuh"
+#include "batch.cuh"
 #include "stream_host.h"
 #include "sample_host.h"
 
@@ -153,26 +153,30 @@ struct nb200_engine {
 
 namespace {
 
-int dmalloc(nb200_engine *e, void **p, size_t bytes) {
+// device memory owned by `allocs` (an engine's, or a batch's: nb200_batch_destroy frees its own)
+int dmalloc_in(std::vector<void *> &allocs, void **p, size_t bytes) {
     if (bytes == 0) bytes = 16;
     cudaError_t err = cudaMalloc(p, bytes);
     if (err != cudaSuccess) return fail(NB200_ENOMEM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(err));
-    e->allocs.push_back(*p);
+    allocs.push_back(*p);
     return 0;
 }
+int dmalloc(nb200_engine *e, void **p, size_t bytes) { return dmalloc_in(e->allocs, p, bytes); }
 #define DM(ptr, bytes) do { int r_ = dmalloc(e, (void **)&(ptr), (bytes)); if (r_) return r_; } while (0)
+#define DMV(allocs, ptr, bytes) do { int r_ = dmalloc_in((allocs), (void **)&(ptr), (bytes)); if (r_) return r_; } while (0)
 
-// b's buffers for m positions; x / xba / hb only where not set already (the exchange block of a tensor-parallel engine)
-int alloc_layer_bufs(nb200_engine *e, LayerBufs &b, uint32_t m) {
+// b's buffers for m positions, owned by allocs; x / xba / hb only where not set already (the exchange block of a
+// tensor-parallel engine)
+int alloc_layer_bufs(nb200_engine *e, std::vector<void *> &allocs, LayerBufs &b, uint32_t m) {
     const Dims &d = e->d;
     const size_t slots = (size_t)m * d.H * e->nsplit_max;
-    if (!b.x) DM(b.x, (size_t)m * d.E * 4);
-    if (!b.xba) DM(b.xba, (size_t)m * d.q_dim * 4);
-    if (!b.hb) DM(b.hb, (size_t)m * d.F * 4);
-    DM(b.q, (size_t)m * d.q_dim * 4); DM(b.kraw, (size_t)m * d.kv_dim * 4);
-    DM(b.ws_m, slots * 4); DM(b.ws_l, slots * 4); DM(b.ws_acc, slots * d.hd * 4);
-    DM(b.tickets, (size_t)m * d.KV * 4); CK(cudaMemset(b.tickets, 0, (size_t)m * d.KV * 4));     // the merging CTA re-zeroes its ticket
-    if (d.exact) DM(b.att, (size_t)m * d.H * d.max_seq * 4);
+    if (!b.x) DMV(allocs, b.x, (size_t)m * d.E * 4);
+    if (!b.xba) DMV(allocs, b.xba, (size_t)m * d.q_dim * 4);
+    if (!b.hb) DMV(allocs, b.hb, (size_t)m * d.F * 4);
+    DMV(allocs, b.q, (size_t)m * d.q_dim * 4); DMV(allocs, b.kraw, (size_t)m * d.kv_dim * 4);
+    DMV(allocs, b.ws_m, slots * 4); DMV(allocs, b.ws_l, slots * 4); DMV(allocs, b.ws_acc, slots * d.hd * 4);
+    DMV(allocs, b.tickets, (size_t)m * d.KV * 4); CK(cudaMemset(b.tickets, 0, (size_t)m * d.KV * 4));     // the merging CTA re-zeroes its ticket
+    if (d.exact) DMV(allocs, b.att, (size_t)m * d.H * d.max_seq * 4);
     return 0;
 }
 
@@ -329,6 +333,7 @@ int run_embed(nb200_engine *e) {
 struct AttnChoice {
     void (*tok)(const AttnArgs);
     void (*pf)(const PrefillAttnArgs);
+    void (*batch)(const BatchAttnArgs);
     uint32_t threads, smem;
     uint32_t kvm;       // fast<KVM>: kv_mul; generic and exact: 0
     uint32_t kind;      // nb200_config.reserved[4] / [6]: 1 exact, 2 generic, 3 | kv_mul << 8 fast
@@ -336,26 +341,27 @@ struct AttnChoice {
 
 AttnChoice pick_attn(const nb200_engine *e) {
     const Dims &d = e->d;
-    if (d.exact) return {nullptr, k_prefill_attention_exact, kAttnThreads, 2 * d.hd * 4, 0u, 1u};
+    if (d.exact) return {nullptr, k_prefill_attention_exact, k_batch_attention_exact, kAttnThreads, 2 * d.hd * 4, 0u, 1u};
     const bool tp = e->tp_size > 1;
     if (d.hd <= 128 && !(d.arch == 3u && (d.hd & (d.hd - 1)) != 0) && (tp || !e->generic_attn)) {
         const uint32_t smem = attn_fast_smem_floats(d.kv_mul, d.hd, e->chunk_cap, e->nsplit_max, kWarps) * 4u;
         switch (d.kv_mul) {
-#define NB_FAST(K) case K: return {tp ? k_attention_fast<K, true> : k_attention_fast<K>, k_prefill_attention_fast<K>, kThreads, smem, K, 3u | (K << 8)};
+#define NB_FAST(K) case K: return {tp ? k_attention_fast<K, true> : k_attention_fast<K>, k_prefill_attention_fast<K>, k_batch_attention_fast<K>, kThreads, smem, K, 3u | (K << 8)};
             NB_FAST(1) NB_FAST(2) NB_FAST(4) NB_FAST(8)
 #undef NB_FAST
             default: break;
         }
     }
-    return {k_attention, k_prefill_attention, kAttnThreads, e->attn_smem, 0u, 2u};
+    return {k_attention, k_prefill_attention, k_batch_attention, kAttnThreads, e->attn_smem, 0u, 2u};
 }
 
-// the attention arguments of layer l over the buffers b (position 0 of b): the split-KV kernels' and the exact kernel's
-void attn_args(const nb200_engine *e, const LayerBufs &b, uint32_t l, AttnArgs &at, AttnExactArgs &ex) {
+// the attention arguments of layer l over the buffers b (position 0 of b) and the K / V cache at kc / vc ([L][KV][max_seq][hd]):
+// the split-KV kernels' and the exact kernel's
+void attn_args(const nb200_engine *e, const LayerBufs &b, float *kc, float *vc, uint32_t l, AttnArgs &at, AttnExactArgs &ex) {
     const Dims &d = e->d;
     const size_t kvl = (size_t)d.KV * d.max_seq * d.hd;
     at = AttnArgs{};
-    at.q = b.q; at.kraw = b.kraw; at.kc = e->kc + l * kvl; at.vc = e->vc + l * kvl;
+    at.q = b.q; at.kraw = b.kraw; at.kc = kc + l * kvl; at.vc = vc + l * kvl;
     at.qnorm = e->qnorm ? e->qnorm + (size_t)l * d.hd : nullptr;
     at.knorm = e->knorm ? e->knorm + (size_t)l * d.hd : nullptr;
     at.rope_cos = e->rope_cos; at.rope_sin = e->rope_sin; at.xba = b.xba;
@@ -395,7 +401,7 @@ int run_layer(nb200_engine *e, uint32_t l) {
         e->prof_tag = 2;
         const AttnChoice ac = pick_attn(e);
         AttnArgs at; AttnExactArgs ex;
-        attn_args(e, b, l, at, ex);
+        attn_args(e, b, e->kc, e->vc, l, at, ex);
         e->attn_kind = ac.kind;
         if (d.exact) r = launch<AttnExactArgs>(e, k_attention_exact, dim3(d.H), dim3(ac.threads), ac.smem, ex);
         else {
@@ -465,23 +471,30 @@ int run_token(nb200_engine *e) {
 }
 
 // ---------------- batched prompt prefill (prefill.cuh) ----------------
-// Chunk size M: the largest value <= kPrefillMax for which M activation operands of the widest matrix, plus the prep's staging
-// copies, fit the shared memory one CTA can get.  The per-position buffers are allocated for M positions on the first call.
-int prefill_setup(nb200_engine *e) {
-    auto &pf = e->pf;
-    if (pf.M) return 0;
+// Chunk size M (prefill, and positions per pass of a batch): the largest value <= kPrefillMax for which M activation operands
+// of the widest matrix, plus the prep's staging copies, fit the shared memory one CTA can get.
+int chunk_positions(nb200_engine *e, uint32_t &M) {
     const Dims &d = e->d;
     int optin = 0;
     CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->device));
     uint32_t maxn = d.E; if (d.q_dim > maxn) maxn = d.q_dim; if (d.F > maxn) maxn = d.F;
     const uint32_t widest = act_region_bytes(d.quant, maxn, d.gs ? d.gs : 1), stage = 2u * maxn * 4u;
     const uint32_t budget = (uint32_t)optin - 256u;        // the kernels' static shared memory (reduction scratch) is 128 bytes
-    uint32_t M = kPrefillMax;
+    M = kPrefillMax;
     while (M > 0 && M * widest + stage > budget) M--;
     if (!M) return fail(NB200_EINVAL, "prefill: one activation operand of %u elements does not fit in shared memory", maxn);
+    return 0;
+}
+
+// The engine's prefill buffers, for M positions, are allocated on the first call.
+int prefill_setup(nb200_engine *e) {
+    auto &pf = e->pf;
+    if (pf.M) return 0;
+    uint32_t M = 0;
     int r;
-    if ((r = alloc_layer_bufs(e, pf.buf, M))) return r;
-    DM(pf.ids, (size_t)d.max_seq * 4);
+    if ((r = chunk_positions(e, M))) return r;
+    if ((r = alloc_layer_bufs(e, e->allocs, pf.buf, M))) return r;
+    DM(pf.ids, (size_t)e->d.max_seq * 4);
     pf.M = M;
     return 0;
 }
@@ -502,12 +515,22 @@ PrefillMvKern prefill_matvec_kernel(const Dims &d) {
     }
 }
 
-// one prefill matvec over the chunk: src / out rows of the m positions are `stride` floats apart
-int run_prefill_matvec(nb200_engine *e, int epi, const Mat &mt, PrefillMvArgs a) {
+// the matrix fields of a chunk matvec over mt (a.m positions) and its launch geometry: returns the dynamic shared memory
+uint32_t chunk_matvec_geometry(const nb200_engine *e, int epi, const Mat &mt, PrefillMvArgs &a, uint32_t &grid) {
     const Dims &d = e->d;
     a.w = mt.w; a.w_aux = mt.aux; a.rows = mt.rows; a.n = mt.n; a.d = d;
     a.act_bytes = act_region_bytes(d.quant, mt.n, d.gs ? d.gs : 1);
-    const uint32_t smem = a.m * a.act_bytes + 2u * mt.n * 4u;
+    if (d.quant == 0x00u && d.exact) grid = ((epi == EPI_SWIGLU ? mt.rows / 2 : mt.rows) + kThreads - 1) / kThreads;
+    else grid = ((mt.rows + kPrefillRB - 1) / kPrefillRB + kWarps - 1) / kWarps;
+    if (grid > (uint32_t)e->num_sms) grid = (uint32_t)e->num_sms;
+    return a.m * a.act_bytes + 2u * mt.n * 4u;
+}
+
+// one prefill matvec over the chunk: src / out rows of the m positions are `stride` floats apart
+int run_prefill_matvec(nb200_engine *e, int epi, const Mat &mt, PrefillMvArgs a) {
+    const Dims &d = e->d;
+    uint32_t grid = 0;
+    const uint32_t smem = chunk_matvec_geometry(e, epi, mt, a, grid);
     PrefillMvKern k = nullptr;
     switch (epi) {
         case EPI_QKV: k = prefill_matvec_kernel<EPI_QKV>(d); break;
@@ -515,18 +538,26 @@ int run_prefill_matvec(nb200_engine *e, int epi, const Mat &mt, PrefillMvArgs a)
         case EPI_SWIGLU: k = prefill_matvec_kernel<EPI_SWIGLU>(d); break;
     }
     if (!k) return fail(NB200_EINVAL, "no prefill matvec kernel for quant=0x%x gs=%u", d.quant, d.gs);
-    uint32_t grid;
-    if (d.quant == 0x00u && d.exact) grid = ((epi == EPI_SWIGLU ? mt.rows / 2 : mt.rows) + kThreads - 1) / kThreads;
-    else grid = ((mt.rows + kPrefillRB - 1) / kPrefillRB + kWarps - 1) / kWarps;
-    if (grid > (uint32_t)e->num_sms) grid = (uint32_t)e->num_sms;
     return launch<PrefillMvArgs>(e, k, dim3(grid), dim3(kThreads), smem, a);
 }
 
-// positions pos0 .. pos0+m-1 (m <= M), ids already on the device
-int run_prefill_chunk(nb200_engine *e, uint32_t pos0, uint32_t m, const uint32_t *ids) {
+// O + residual, W1|W3 + SwiGLU, W2 + residual of layer l for m positions of b (prefill chunks and batch passes)
+int run_chunk_ffn(nb200_engine *e, const LayerBufs &b, uint32_t l, uint32_t pos0, uint32_t m) {
     const Dims &d = e->d;
-    auto &pf = e->pf;
-    const LayerBufs &b = pf.buf;
+    int r;
+    PrefillMvArgs a{};
+    a.pos0 = pos0; a.m = m;
+    a.src = b.xba; a.src_stride = d.q_dim; a.out = b.x; a.out_stride = d.E;
+    if ((r = run_prefill_matvec(e, EPI_RESID, e->wo[l], a))) return r;
+    a.src = b.x; a.src_stride = d.E; a.gain = e->norm_ffn + (size_t)l * d.E; a.out = b.hb; a.out_stride = d.F;
+    if ((r = run_prefill_matvec(e, EPI_SWIGLU, e->w13[l], a))) return r;
+    a.src = b.hb; a.src_stride = d.F; a.gain = nullptr; a.out = b.x; a.out_stride = d.E;
+    return run_prefill_matvec(e, EPI_RESID, e->w2[l], a);
+}
+
+// positions pos0 .. pos0+m-1 (m <= M) into the K / V cache at kc / vc over the buffers b, ids already on the device
+int run_prefill_chunk(nb200_engine *e, float *kc, float *vc, const LayerBufs &b, uint32_t pos0, uint32_t m, const uint32_t *ids) {
+    const Dims &d = e->d;
     const size_t kvl = (size_t)d.KV * d.max_seq * d.hd;
     const AttnChoice ac = pick_attn(e);
     int r;
@@ -538,27 +569,19 @@ int run_prefill_chunk(nb200_engine *e, uint32_t pos0, uint32_t m, const uint32_t
         PrefillMvArgs a{};
         a.pos0 = pos0; a.m = m;
         a.src = b.x; a.src_stride = d.E; a.gain = e->norm_attn + (size_t)l * d.E;
-        a.out = b.q; a.out_stride = d.q_dim; a.out_k = b.kraw; a.k_stride = d.kv_dim; a.out_v = e->vc + l * kvl;
+        a.out = b.q; a.out_stride = d.q_dim; a.out_k = b.kraw; a.k_stride = d.kv_dim; a.out_v = vc + l * kvl;
         if ((r = run_prefill_matvec(e, EPI_QKV, e->qkv[l], a))) return r;
 
         PrefillAttnArgs pa{};
         pa.pos0 = pos0;
-        attn_args(e, b, l, pa.at, pa.ex);
+        attn_args(e, b, kc, vc, l, pa.at, pa.ex);
         PrefillKrowArgs kr{b.kraw, pa.at.kc, pa.at.knorm, e->rope_cos, e->rope_sin, pos0, ac.kvm ? 1u : 0u, d};
         if ((r = launch<PrefillKrowArgs>(e, k_prefill_krow, dim3(d.KV, m), dim3(32), 0, kr))) return r;
 
-        pf.attn_kind = ac.kind;
         const dim3 grid = d.exact ? dim3(d.H, m) : dim3(e->nsplit_max, d.KV, m);
         if ((r = launch<PrefillAttnArgs>(e, ac.pf, grid, dim3(ac.threads), ac.smem, pa))) return r;
 
-        a = PrefillMvArgs{};
-        a.pos0 = pos0; a.m = m;
-        a.src = b.xba; a.src_stride = d.q_dim; a.out = b.x; a.out_stride = d.E;
-        if ((r = run_prefill_matvec(e, EPI_RESID, e->wo[l], a))) return r;
-        a.src = b.x; a.src_stride = d.E; a.gain = e->norm_ffn + (size_t)l * d.E; a.out = b.hb; a.out_stride = d.F;
-        if ((r = run_prefill_matvec(e, EPI_SWIGLU, e->w13[l], a))) return r;
-        a.src = b.hb; a.src_stride = d.F; a.gain = nullptr; a.out = b.x; a.out_stride = d.E;
-        if ((r = run_prefill_matvec(e, EPI_RESID, e->w2[l], a))) return r;
+        if ((r = run_chunk_ffn(e, b, l, pos0, m))) return r;
     }
     return 0;
 }
@@ -1080,7 +1103,7 @@ static int create_impl(nb200_engine **out, const uint8_t *img, uint64_t image_by
     uint32_t lpr = 1; while (lpr * 4 < d.hd) lpr <<= 1; if (lpr > 32) lpr = 32;
     const uint32_t rpw = 32 / lpr;
     e->attn_smem = (uint32_t)((d.kv_mul * d.hd + d.hd + cap + (size_t)kAttnWarps * rpw * d.hd) * 4);
-    if ((r = alloc_layer_bufs(e, e->buf, 1))) return r;
+    if ((r = alloc_layer_bufs(e, e->allocs, e->buf, 1))) return r;
     CK(cudaMemset(e->buf.x, 0, E * 4));
     DM(e->ids_dev, ((size_t)d.max_seq + 8) * 4); CK(cudaMemset(e->ids_dev, 0, ((size_t)d.max_seq + 8) * 4));
     DM(e->seen, V); CK(cudaMemset(e->seen, 0, V));
@@ -1358,22 +1381,29 @@ int nb200_read_logits(nb200_engine *e, float *host_logits) {
     return 0;
 }
 
-static int sync_seen(nb200_engine *e, const uint32_t *ids, uint32_t pos) {
-    uint32_t have = (uint32_t)e->seen_mirror.size();
-    bool ok = e->seen_valid && have <= pos && (have == 0 || memcmp(e->seen_mirror.data(), ids, (size_t)have * 4) == 0);
+// Bring a seen set ([V] flags, device ids copy ids_dev) to ids[0..pos): the host mirror records the ids it was marked from, so
+// a continued session marks only its new ids and a rewind or a new session clears the set first.
+static int sync_seen_set(nb200_engine *e, uint8_t *seen, uint32_t *ids_dev, std::vector<uint32_t> &mirror, bool &valid,
+                         const uint32_t *ids, uint32_t pos) {
+    uint32_t have = (uint32_t)mirror.size();
+    bool ok = valid && have <= pos && (have == 0 || memcmp(mirror.data(), ids, (size_t)have * 4) == 0);
     if (!ok) {
-        CK(cudaMemsetAsync(e->seen, 0, e->d.V, e->stream));
-        e->seen_mirror.clear(); have = 0; e->seen_valid = true;
+        CK(cudaMemsetAsync(seen, 0, e->d.V, e->stream));
+        mirror.clear(); have = 0; valid = true;
     }
     if (pos > have) {
         for (uint32_t i = have; i < pos; i++) if (ids[i] >= e->d.V) return fail(NB200_EINVAL, "id out of range");
-        CK(cudaMemcpyAsync(e->ids_dev + have, ids + have, (size_t)(pos - have) * 4, cudaMemcpyHostToDevice, e->stream));
-        k_mark_seen<<<1, 256, 0, e->stream>>>(e->seen, e->ids_dev, have, pos);
+        CK(cudaMemcpyAsync(ids_dev + have, ids + have, (size_t)(pos - have) * 4, cudaMemcpyHostToDevice, e->stream));
+        k_mark_seen<<<1, 256, 0, e->stream>>>(seen, ids_dev, have, pos);
         CK(cudaGetLastError());
         e->launches++;
-        e->seen_mirror.insert(e->seen_mirror.end(), ids + have, ids + pos);
+        mirror.insert(mirror.end(), ids + have, ids + pos);
     }
     return 0;
+}
+
+static int sync_seen(nb200_engine *e, const uint32_t *ids, uint32_t pos) {
+    return sync_seen_set(e, e->seen, e->ids_dev, e->seen_mirror, e->seen_valid, ids, pos);
 }
 
 int nb200_next_greedy(nb200_engine *e, const uint32_t *ids, uint32_t pos, int is_prefilling, float penalty, uint32_t *next) {
@@ -1464,15 +1494,276 @@ int nb200_prefill(nb200_engine *e, const uint32_t *ids, uint32_t pos0, uint32_t 
     for (auto &v : evs.ev) CK(cudaEventCreate(&v));
     CK(cudaMemcpyAsync(e->pf.ids, ids + pos0, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
     CK(cudaEventRecord(evs.ev[0], e->stream));
+    e->pf.attn_kind = pick_attn(e).kind;
     for (uint32_t c = 0; c < n; c += e->pf.M) {
         const uint32_t m = (n - c < e->pf.M) ? n - c : e->pf.M;
-        if ((r = run_prefill_chunk(e, pos0 + c, m, e->pf.ids + c))) return r;
+        if ((r = run_prefill_chunk(e, e->kc, e->vc, e->pf.buf, pos0 + c, m, e->pf.ids + c))) return r;
     }
     CK(cudaEventRecord(evs.ev[1], e->stream));
     CK(cudaStreamSynchronize(e->stream));
     float ms = 0.0f;
     CK(cudaEventElapsedTime(&ms, evs.ev[0], evs.ev[1]));
     if (device_ms) *device_ms = ms;
+    return 0;
+}
+
+}  // extern "C"
+
+// ---------------- batched multi-session decode (batch.cuh) ----------------
+// A batch shares its engine's weights, norms and RoPE tables and owns everything that belongs to a session: per slot a K / V
+// cache laid out like the engine's, a logits row, a seen set with its host mirror and device ids copy.  The per-position
+// buffers of a pass (M positions) and the pass records are the batch's own too, so the engine's state is never touched.
+struct nb200_batch {
+    nb200_engine *e = nullptr;
+    uint32_t n_slots = 0, M = 0, attn_kind = 0, max_pass = 0;
+    size_t slot_elems = 0;                    // floats of one slot's K (or V) cache: L * KV * max_seq * hd
+    float *kc = nullptr, *vc = nullptr;       // [n_slots][L][KV][max_seq][hd]
+    float *logits = nullptr;                  // [n_slots][V]
+    uint8_t *seen = nullptr;                  // [n_slots][V]
+    uint32_t *ids = nullptr;                  // [n_slots][max_seq]: the ids each slot's seen set was marked from
+    uint32_t *pf_ids = nullptr;               // [max_seq]: ids of the running nb200_batch_prefill
+    std::vector<BatchPass> pass_host;         // [max_pass]
+    uint32_t *ids_pass = nullptr, *ids_pass_host = nullptr;   // [n_slots] the ids the entries consume, the host copy pinned
+    uint32_t *next_dev = nullptr, *next_host = nullptr;       // [n_slots] result ids, the host copy pinned
+    LayerBufs buf;                            // M positions
+    std::vector<std::vector<uint32_t>> mirror;
+    std::vector<char> mirror_valid;
+    std::vector<void *> allocs;
+};
+
+namespace {
+
+int batch_usable(const nb200_batch *b) {
+    if (!b) return fail(NB200_EINVAL, "null batch");
+    if (b->e->tp_size > 1) return fail(NB200_EINVAL, "batches are not available on tensor-parallel engines");
+    if (b->e->lora.active) return fail(NB200_EINVAL, "batches do not run LoRA plug-ins: disable the plug-in (nb200_lora_enable)");
+    return 0;
+}
+
+// the QKV (EPI_QKV) or classifier (EPI_CLS) matvec of a pass
+typedef void (*BatchMvKern)(const BatchMvArgs);
+template <int EPI>
+BatchMvKern batch_matvec_kernel(const Dims &d) {
+    constexpr int RB = kPrefillRB;
+    if (d.quant == 0x00u) return d.exact ? k_batch_matvec_f32_exact<EPI> : k_batch_matvec<0x00, EPI, RB, 8>;
+    if (d.quant == 0x42u) return k_batch_matvec<0x42, EPI, RB, 8>;
+    switch (matvec_lpg(d)) {
+        case 2: return k_batch_matvec<0x80, EPI, RB, 2>;
+        case 4: return k_batch_matvec<0x80, EPI, RB, 4>;
+        case 8: return k_batch_matvec<0x80, EPI, RB, 8>;
+        case 16: return k_batch_matvec<0x80, EPI, RB, 16>;
+        default: return nullptr;
+    }
+}
+
+int run_batch_matvec(nb200_engine *e, int epi, const Mat &mt, BatchMvArgs a) {
+    const Dims &d = e->d;
+    uint32_t grid = 0;
+    const uint32_t smem = chunk_matvec_geometry(e, epi, mt, a.mv, grid);
+    BatchMvKern k = (epi == EPI_QKV) ? batch_matvec_kernel<EPI_QKV>(d) : batch_matvec_kernel<EPI_CLS>(d);
+    if (!k) return fail(NB200_EINVAL, "no batch matvec kernel for quant=0x%x gs=%u", d.quant, d.gs);
+    return launch<BatchMvArgs>(e, k, dim3(grid), dim3(kThreads), smem, a);
+}
+
+// one pass: the m entries of bp (their ids also at ids on the device) -> their slots' K / V rows and logits, next ids at next[0..m)
+int run_batch_pass(nb200_batch *b, const BatchPass &bp, const uint32_t *ids, uint32_t m, uint32_t *next) {
+    nb200_engine *e = b->e;
+    const Dims &d = e->d;
+    const LayerBufs &buf = b->buf;
+    const size_t kvl = (size_t)d.KV * d.max_seq * d.hd;
+    const AttnChoice ac = pick_attn(e);
+    int r;
+    {
+        PrefillEmbedArgs a{e->emb.w, e->emb.aux, buf.x, ids, d};
+        if ((r = launch<PrefillEmbedArgs>(e, k_prefill_embed, dim3(m), dim3(256), 0, a))) return r;
+    }
+    for (uint32_t l = 0; l < d.L; l++) {
+        BatchMvArgs a{};
+        a.mv.m = m;
+        a.mv.src = buf.x; a.mv.src_stride = d.E; a.mv.gain = e->norm_attn + (size_t)l * d.E;
+        a.mv.out = buf.q; a.mv.out_stride = d.q_dim; a.mv.out_k = buf.kraw; a.mv.k_stride = d.kv_dim;
+        a.bp = bp; a.vc = b->vc + l * kvl; a.slot_elems = b->slot_elems;
+        if ((r = run_batch_matvec(e, EPI_QKV, e->qkv[l], a))) return r;
+
+        BatchAttnArgs ba{};
+        attn_args(e, buf, b->kc, b->vc, l, ba.pa.at, ba.pa.ex);
+        ba.bp = bp; ba.slot_elems = b->slot_elems;
+        const dim3 grid = d.exact ? dim3(d.H, m) : dim3(e->nsplit_max, d.KV, m);
+        if ((r = launch<BatchAttnArgs>(e, ac.batch, grid, dim3(ac.threads), ac.smem, ba))) return r;
+
+        if ((r = run_chunk_ffn(e, buf, l, 0, m))) return r;
+    }
+    BatchMvArgs a{};
+    a.mv.m = m;
+    a.mv.src = buf.x; a.mv.src_stride = d.E; a.mv.gain = e->norm_final;
+    a.bp = bp; a.logits = b->logits; a.seen = b->seen;
+    if ((r = run_batch_matvec(e, EPI_CLS, e->cls, a))) return r;
+    BatchArgmaxArgs am{b->logits, bp, next, d.V};
+    return launch<BatchArgmaxArgs>(e, k_batch_argmax, dim3(m), dim3(1024), 0, am);
+}
+
+}  // namespace
+
+extern "C" {
+
+void nb200_batch_destroy(nb200_batch *b) {
+    if (!b) return;
+    cudaSetDevice(b->e->device);
+    cudaStreamSynchronize(b->e->stream);
+    for (void *p : b->allocs) cudaFree(p);
+    if (b->ids_pass_host) cudaFreeHost(b->ids_pass_host);
+    if (b->next_host) cudaFreeHost(b->next_host);
+    delete b;
+}
+
+int nb200_batch_create(nb200_engine *e, uint32_t n_slots, nb200_batch **out) {
+    if (!e || !out) return fail(NB200_EINVAL, "null argument");
+    *out = nullptr;
+    if (e->tp_size > 1) return fail(NB200_EINVAL, "batches are not available on tensor-parallel engines");
+    if (e->lora.active) return fail(NB200_EINVAL, "batches do not run LoRA plug-ins: disable the plug-in (nb200_lora_enable)");
+    if (n_slots == 0) return fail(NB200_EINVAL, "a batch needs at least one slot");
+    CK(cudaSetDevice(e->device));
+    const Dims &d = e->d;
+    nb200_batch *b = new nb200_batch;
+    b->e = e; b->n_slots = n_slots;
+    b->mirror.resize(n_slots); b->mirror_valid.assign(n_slots, 0);
+    int r = chunk_positions(e, b->M);
+    auto init = [&]() -> int {
+        b->attn_kind = pick_attn(e).kind;
+        b->max_pass = (n_slots + b->M - 1) / b->M;
+        b->slot_elems = (size_t)d.L * d.KV * d.max_seq * d.hd;
+        const size_t kv_bytes = (size_t)n_slots * b->slot_elems * 4;
+        DMV(b->allocs, b->kc, kv_bytes); DMV(b->allocs, b->vc, kv_bytes);
+        CK(cudaMemset(b->kc, 0, kv_bytes)); CK(cudaMemset(b->vc, 0, kv_bytes));
+        DMV(b->allocs, b->logits, (size_t)n_slots * d.V * 4); CK(cudaMemset(b->logits, 0, (size_t)n_slots * d.V * 4));
+        DMV(b->allocs, b->seen, (size_t)n_slots * d.V); CK(cudaMemset(b->seen, 0, (size_t)n_slots * d.V));
+        DMV(b->allocs, b->ids, (size_t)n_slots * d.max_seq * 4);
+        DMV(b->allocs, b->pf_ids, (size_t)d.max_seq * 4);
+        DMV(b->allocs, b->ids_pass, (size_t)n_slots * 4);
+        b->pass_host.resize(b->max_pass);
+        DMV(b->allocs, b->next_dev, (size_t)n_slots * 4);
+        CK(cudaHostAlloc(&b->ids_pass_host, (size_t)n_slots * 4, cudaHostAllocDefault));
+        CK(cudaHostAlloc(&b->next_host, (size_t)n_slots * 4, cudaHostAllocDefault));
+        return alloc_layer_bufs(e, b->allocs, b->buf, b->M);
+    };
+    if (!r) r = init();
+    if (r) { nb200_batch_destroy(b); return r; }
+    *out = b;
+    return 0;
+}
+
+int nb200_batch_info(const nb200_batch *b, uint32_t info[4]) {
+    if (!b || !info) return fail(NB200_EINVAL, "null argument");
+    info[0] = b->M; info[1] = b->n_slots; info[2] = b->attn_kind; info[3] = 0;
+    return 0;
+}
+
+int nb200_batch_prefill(nb200_batch *b, uint32_t slot, const uint32_t *ids, uint32_t pos0, uint32_t n, float *device_ms) {
+    int r;
+    if ((r = batch_usable(b))) return r;
+    nb200_engine *e = b->e;
+    if (!ids) return fail(NB200_EINVAL, "null argument");
+    if (slot >= b->n_slots) return fail(NB200_EINVAL, "slot %u of a batch of %u", slot, b->n_slots);
+    const uint32_t lim = pos_limit(e->d);
+    if (n == 0 || pos0 >= lim || n > lim - pos0)
+        return fail(NB200_EINVAL, "prefill of %u positions from %u: empty, or past min(max_seq_len, block_size) = %u", n, pos0, lim);
+    for (uint32_t p = pos0; p < pos0 + n; p++) if (ids[p] >= e->d.V) return fail(NB200_EINVAL, "id %u at position %u out of range", ids[p], p);
+    CK(cudaSetDevice(e->device));
+    struct Events { cudaEvent_t ev[2] = {nullptr, nullptr}; ~Events() { for (auto v : ev) if (v) cudaEventDestroy(v); } } evs;
+    for (auto &v : evs.ev) CK(cudaEventCreate(&v));
+    CK(cudaMemcpyAsync(b->pf_ids, ids + pos0, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaEventRecord(evs.ev[0], e->stream));
+    float *kc = b->kc + slot * b->slot_elems, *vc = b->vc + slot * b->slot_elems;
+    for (uint32_t c = 0; c < n; c += b->M) {
+        const uint32_t m = (n - c < b->M) ? n - c : b->M;
+        if ((r = run_prefill_chunk(e, kc, vc, b->buf, pos0 + c, m, b->pf_ids + c))) return r;
+    }
+    CK(cudaEventRecord(evs.ev[1], e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    float ms = 0.0f;
+    CK(cudaEventElapsedTime(&ms, evs.ev[0], evs.ev[1]));
+    if (device_ms) *device_ms = ms;
+    return 0;
+}
+
+int nb200_batch_next_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t *const *ids, const uint32_t *pos,
+                            const float *repetition_penalty, uint32_t *next_tokens, float *device_ms) {
+    int r;
+    if ((r = batch_usable(b))) return r;
+    nb200_engine *e = b->e;
+    const Dims &d = e->d;
+    if (!slots || !ids || !pos || !repetition_penalty || !next_tokens) return fail(NB200_EINVAL, "null argument");
+    if (n == 0) return fail(NB200_EINVAL, "no entries");
+    // every check before anything is written
+    std::vector<char> used(b->n_slots, 0);
+    const uint32_t lim = pos_limit(d);
+    for (uint32_t i = 0; i < n; i++) {
+        if (slots[i] >= b->n_slots) return fail(NB200_EINVAL, "entry %u: slot %u of a batch of %u", i, slots[i], b->n_slots);
+        if (used[slots[i]]) return fail(NB200_EINVAL, "entry %u: slot %u appears twice in one call", i, slots[i]);
+        used[slots[i]] = 1;
+        if (!ids[i]) return fail(NB200_EINVAL, "entry %u: null ids", i);
+        if (pos[i] >= lim) return fail(NB200_EINVAL, "entry %u: position %u past min(max_seq_len, block_size) = %u", i, pos[i], lim);
+        const uint32_t upto = (repetition_penalty[i] != 1.0f) ? 0 : pos[i];      // the penalty reads ids[0..pos)
+        for (uint32_t p = upto; p <= pos[i]; p++)
+            if (ids[i][p] >= d.V) return fail(NB200_EINVAL, "entry %u: id %u at position %u out of range", i, ids[i][p], p);
+    }
+    CK(cudaSetDevice(e->device));
+    struct Events { cudaEvent_t ev[2] = {nullptr, nullptr}; ~Events() { for (auto v : ev) if (v) cudaEventDestroy(v); } } evs;
+    for (auto &v : evs.ev) CK(cudaEventCreate(&v));
+    CK(cudaStreamSynchronize(e->stream));           // the pinned ids and results may still be in flight
+    const uint32_t npass = (n + b->M - 1) / b->M;
+    for (uint32_t i = 0; i < n; i++) {
+        BatchPass &ps = b->pass_host[i / b->M];
+        const uint32_t p = i % b->M;
+        ps.slot[p] = slots[i]; ps.pos[p] = pos[i]; ps.pen[p] = repetition_penalty[i];
+        b->ids_pass_host[i] = ids[i][pos[i]];
+    }
+    CK(cudaEventRecord(evs.ev[0], e->stream));
+    for (uint32_t i = 0; i < n; i++) {
+        if (repetition_penalty[i] == 1.0f) continue;       // x / 1.0f == x: the classifier skips the lookup, as nb200_next_greedy
+        const uint32_t s = slots[i];
+        bool valid = b->mirror_valid[s] != 0;
+        r = sync_seen_set(e, b->seen + (size_t)s * d.V, b->ids + (size_t)s * d.max_seq, b->mirror[s], valid, ids[i], pos[i]);
+        b->mirror_valid[s] = valid ? 1 : 0;
+        if (r) return r;
+    }
+    CK(cudaMemcpyAsync(b->ids_pass, b->ids_pass_host, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+    for (uint32_t k = 0; k < npass; k++) {
+        const uint32_t m = (n - k * b->M < b->M) ? n - k * b->M : b->M;
+        if ((r = run_batch_pass(b, b->pass_host[k], b->ids_pass + k * b->M, m, b->next_dev + k * b->M))) return r;
+    }
+    CK(cudaEventRecord(evs.ev[1], e->stream));
+    CK(cudaMemcpyAsync(b->next_host, b->next_dev, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    memcpy(next_tokens, b->next_host, (size_t)n * 4);
+    float ms = 0.0f;
+    CK(cudaEventElapsedTime(&ms, evs.ev[0], evs.ev[1]));
+    if (device_ms) *device_ms = ms;
+    return 0;
+}
+
+int nb200_batch_read_logits(nb200_batch *b, uint32_t slot, float *host_logits) {
+    if (!b || !host_logits) return fail(NB200_EINVAL, "null argument");
+    if (slot >= b->n_slots) return fail(NB200_EINVAL, "slot %u of a batch of %u", slot, b->n_slots);
+    nb200_engine *e = b->e;
+    CK(cudaSetDevice(e->device));
+    CK(cudaMemcpyAsync(host_logits, b->logits + (size_t)slot * e->d.V, (size_t)e->d.V * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    return 0;
+}
+
+int nb200_batch_read_kv(nb200_batch *b, uint32_t slot, int field, uint32_t layer, uint32_t pos, float *dst, uint32_t count) {
+    if (!b || !dst) return fail(NB200_EINVAL, "null argument");
+    nb200_engine *e = b->e;
+    const Dims &d = e->d;
+    if (slot >= b->n_slots) return fail(NB200_EINVAL, "slot %u of a batch of %u", slot, b->n_slots);
+    if (field != NB200_F_KROW && field != NB200_F_VROW) return fail(NB200_EINVAL, "a batch holds K and V rows only (field %d)", field);
+    if (layer >= d.L || pos >= d.max_seq || count != d.kv_dim) return fail(NB200_EINVAL, "bad KV row request");
+    CK(cudaSetDevice(e->device));
+    CK(cudaStreamSynchronize(e->stream));
+    const float *base = (field == NB200_F_KROW ? b->kc : b->vc) + slot * b->slot_elems + (size_t)layer * d.KV * d.max_seq * d.hd;
+    for (uint32_t h = 0; h < d.KV; h++)
+        CK(cudaMemcpy(dst + (size_t)h * d.hd, base + ((size_t)h * d.max_seq + pos) * d.hd, (size_t)d.hd * 4, cudaMemcpyDeviceToHost));
     return 0;
 }
 

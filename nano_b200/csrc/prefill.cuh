@@ -92,15 +92,11 @@ __device__ __forceinline__ void prefill_rows_q80(const PrefillMvArgs &a, uint32_
     }
 }
 
-// rmsnorm / quantise of every position's input into its own operand, then row blocks x positions.
+// rmsnorm / quantise of every position's input into its own operand, then row blocks x positions; store(p, row0, val) finishes
+// the RB rows from row0 of position p (k_prefill_matvec: prefill_store; the batch kernels of batch.cuh: their own stores).
 // smem: m activation operands of act_bytes each | staging (2n floats, reused by every position's prep)
-template <int QUANT, int EPI, int RB, int LPG>
-__global__ void __launch_bounds__(kThreads, 1) k_prefill_matvec(const PrefillMvArgs a) {
-    extern __shared__ __align__(16) unsigned char act[];
-    __shared__ float red[32];
-    pdl_launch_dependents();
-    prefetch_row_blocks<QUANT, RB>(a.w, a.rows, a.n, blockIdx.x, gridDim.x, 4);
-    pdl_wait();
+template <int QUANT, int RB, int LPG, class Store>
+__device__ __forceinline__ void prefill_matvec_body(const PrefillMvArgs &a, unsigned char *act, float *red, Store &&store) {
     const bool exact = a.d.exact != 0;
     const uint32_t n = a.n;
     float *stage = reinterpret_cast<float *>(act + (size_t)a.m * a.act_bytes);
@@ -131,35 +127,53 @@ __global__ void __launch_bounds__(kThreads, 1) k_prefill_matvec(const PrefillMvA
             }
 #pragma unroll
             for (int p = 0; p < kPrefillMax; p++)
-                if (p < (int)a.m) prefill_store<EPI, RB>(a, p, row0, val[p]);
+                if (p < (int)a.m) store((uint32_t)p, row0, val[p]);
         } else {
             for (uint32_t p = 0; p < a.m; p++) {
                 float val[RB];
                 const unsigned char *ap = act + (size_t)p * a.act_bytes;
                 if (QUANT == 0x00) rows_f32<RB>(static_cast<const float *>(a.w), row0, a.rows, n, ap, val);
                 else rows_q4k<RB>(static_cast<const uint8_t *>(a.w), static_cast<const uint8_t *>(a.w_aux), row0, a.rows, n, ap, val);
-                prefill_store<EPI, RB>(a, p, row0, val);
+                store(p, row0, val);
             }
         }
     }
 }
 
-// exact-mode F32 (k_matvec_f32_exact over the chunk): one thread per unit, f32_exact_unit per position
-template <int EPI>
-__global__ void __launch_bounds__(kThreads, 1) k_prefill_matvec_f32_exact(const PrefillMvArgs a) {
+template <int QUANT, int EPI, int RB, int LPG>
+__global__ void __launch_bounds__(kThreads, 1) k_prefill_matvec(const PrefillMvArgs a) {
     extern __shared__ __align__(16) unsigned char act[];
     __shared__ float red[32];
     pdl_launch_dependents();
+    prefetch_row_blocks<QUANT, RB>(a.w, a.rows, a.n, blockIdx.x, gridDim.x, 4);
     pdl_wait();
+    prefill_matvec_body<QUANT, RB, LPG>(a, act, red, [&](uint32_t p, uint32_t row0, const float (&val)[RB]) { prefill_store<EPI, RB>(a, p, row0, val); });
+}
+
+// exact-mode F32 over the chunk (k_matvec_f32_exact's arithmetic): every position's operand, then unit(p, u, x) for unit u of
+// every position p, one thread per unit (a row, or a w1 / w3 row pair for EPI_SWIGLU)
+template <int EPI, class Unit>
+__device__ __forceinline__ void prefill_f32_exact_body(const PrefillMvArgs &a, unsigned char *act, float *red, Unit &&unit) {
     const uint32_t n = a.n;
     float *stage = reinterpret_cast<float *>(act + (size_t)a.m * a.act_bytes);
     for (uint32_t p = 0; p < a.m; p++)
         prep_f32<kThreads>(a.src + (size_t)p * a.src_stride, a.gain, n, true, reinterpret_cast<float *>(act + (size_t)p * a.act_bytes), stage, red);
     const uint32_t nunits = (EPI == EPI_SWIGLU) ? a.rows / 2 : a.rows;
     for (uint32_t u = blockIdx.x * kThreads + threadIdx.x; u < nunits; u += gridDim.x * kThreads)
-        for (uint32_t p = 0; p < a.m; p++)
-            f32_exact_unit<EPI>(static_cast<const float *>(a.w), n, u, reinterpret_cast<const float *>(act + (size_t)p * a.act_bytes), a.d,
-                                a.out + (size_t)p * a.out_stride, a.out_k + (size_t)p * a.k_stride, a.out_v, a.pos0 + p, nullptr);
+        for (uint32_t p = 0; p < a.m; p++) unit(p, u, reinterpret_cast<const float *>(act + (size_t)p * a.act_bytes));
+}
+
+// exact-mode F32 (k_matvec_f32_exact over the chunk): f32_exact_unit per position
+template <int EPI>
+__global__ void __launch_bounds__(kThreads, 1) k_prefill_matvec_f32_exact(const PrefillMvArgs a) {
+    extern __shared__ __align__(16) unsigned char act[];
+    __shared__ float red[32];
+    pdl_launch_dependents();
+    pdl_wait();
+    prefill_f32_exact_body<EPI>(a, act, red, [&](uint32_t p, uint32_t u, const float *x) {
+        f32_exact_unit<EPI>(static_cast<const float *>(a.w), a.n, u, x, a.d, a.out + (size_t)p * a.out_stride,
+                            a.out_k + (size_t)p * a.k_stride, a.out_v, a.pos0 + p, nullptr);
+    });
 }
 
 // the embedding rows of the chunk's ids (embed_row, as k_embed), one CTA per position
@@ -250,17 +264,20 @@ NB_K __global__ void __launch_bounds__(kAttnThreads, 1) k_prefill_attention(cons
     attn_generic_cta(prefill_attn_at(pa, p), blockIdx.y, blockIdx.x, pos, pos + 1, sm, red, is_last);
 }
 
+__device__ __forceinline__ AttnExactArgs prefill_exact_at(const PrefillAttnArgs &pa, uint32_t p) {
+    AttnExactArgs a = pa.ex;
+    const Dims &d = a.d;
+    a.q += (size_t)p * d.q_dim; a.kraw += (size_t)p * d.kv_dim; a.xba += (size_t)p * d.q_dim;
+    a.att += (size_t)p * d.H * d.max_seq;
+    return a;
+}
 NB_K __global__ void __launch_bounds__(kAttnThreads) k_prefill_attention_exact(const PrefillAttnArgs pa) {
     extern __shared__ __align__(16) float sm[];
     __shared__ float red[32];
     pdl_launch_dependents();
     pdl_wait();
     const uint32_t p = blockIdx.y, pos = pa.pos0 + p;
-    AttnExactArgs a = pa.ex;
-    const Dims &d = a.d;
-    a.q += (size_t)p * d.q_dim; a.kraw += (size_t)p * d.kv_dim; a.xba += (size_t)p * d.q_dim;
-    a.att += (size_t)p * d.H * d.max_seq;
-    attn_exact_cta(a, blockIdx.x, pos, pos + 1, sm, red);
+    attn_exact_cta(prefill_exact_at(pa, p), blockIdx.x, pos, pos + 1, sm, red);
 }
 
 }  // namespace nb

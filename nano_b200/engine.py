@@ -32,6 +32,8 @@ EXPORTS = [
     "nb200_op_q4k_quantize_blocks", "nb200_op_q4k_matvec_blocks",
     "nb200_lora_load", "nb200_lora_enable", "nb200_lora_unload",
     "nb200_engine_create_tp", "nb200_tp_export", "nb200_tp_attach_ipc", "nb200_tp_attach_local",
+    "nb200_batch_create", "nb200_batch_destroy", "nb200_batch_prefill", "nb200_batch_next_greedy", "nb200_batch_read_logits",
+    "nb200_batch_read_kv", "nb200_batch_info",
 ]
 
 
@@ -94,6 +96,13 @@ def lib():
         L.nb200_lora_load.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
         L.nb200_lora_enable.argtypes = [C.c_void_p, C.c_int]
         L.nb200_lora_unload.argtypes = [C.c_void_p]
+        L.nb200_batch_create.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p)]
+        L.nb200_batch_destroy.argtypes = [C.c_void_p]
+        L.nb200_batch_prefill.argtypes = [C.c_void_p, C.c_uint32, u32p, C.c_uint32, C.c_uint32, f32p]
+        L.nb200_batch_next_greedy.argtypes = [C.c_void_p, C.c_uint32, u32p, C.POINTER(u32p), u32p, f32p, u32p, f32p]
+        L.nb200_batch_read_logits.argtypes = [C.c_void_p, C.c_uint32, f32p]
+        L.nb200_batch_read_kv.argtypes = [C.c_void_p, C.c_uint32, C.c_int, C.c_uint32, C.c_uint32, f32p, C.c_uint32]
+        L.nb200_batch_info.argtypes = [C.c_void_p, u32p]
         L.nb200_host_expf_ref.restype = C.c_float
         L.nb200_host_expf_ref.argtypes = [C.c_float]
         L.nb200_host_expf_ref_array.argtypes = [f32p, f32p, C.c_uint64]
@@ -129,6 +138,7 @@ class Engine:
         else:
             image = np.frombuffer(bytes(model), dtype=np.uint8)
         self.h = C.c_void_p()
+        self._batches = []
         if tp is None:
             _check(L.nb200_engine_create(C.byref(self.h), image.ctypes.data, image.size, max_seq, device, flags))
         else:
@@ -200,8 +210,16 @@ class Engine:
         per = self.vocab // self.tp_size
         return self.tp_rank * per, (self.tp_rank + 1) * per
 
+    def batch(self, n_slots: int) -> "Batch":
+        """A batch of n_slots independent sessions decoded together over this engine's weights (nb200_batch_*)."""
+        b = Batch(self, n_slots)
+        self._batches.append(b)
+        return b
+
     def close(self):
         if getattr(self, "h", None):
+            for b in list(getattr(self, "_batches", [])):      # a batch must go before its engine
+                b.close()
             lib().nb200_engine_destroy(self.h)
             self.h = None
 
@@ -292,6 +310,69 @@ class Engine:
     @property
     def weight_bytes(self) -> int:
         return int(lib().nb200_weight_bytes(self.h))
+
+
+class Batch:
+    """Up to n_slots sessions sharing one engine's weights; each slot has its own K / V cache, seen set and logits
+    (include/nano_b200.h, nb200_batch_*).  Create it with Engine.batch; Engine.close closes it first."""
+
+    def __init__(self, engine: Engine, n_slots: int):
+        self.engine = engine
+        self.h = C.c_void_p()
+        _check(lib().nb200_batch_create(engine.h, int(n_slots), C.byref(self.h)))
+        self.device_ms = 0.0        # device time of the last next_greedy
+
+    def info(self) -> dict:
+        """{"chunk": positions per pass M, "slots": n_slots, "attention": the attention kernel, named as Engine.kernels()}"""
+        out = np.zeros(4, np.uint32)
+        _check(lib().nb200_batch_info(self.h, _p(out, u32p)))
+        return {"chunk": int(out[0]), "slots": int(out[1]), "attention": _attention_kind(int(out[2]))}
+
+    def prefill(self, slot: int, ids: np.ndarray, pos0: int, n: int) -> float:
+        """Engine.prefill into one slot's cache; returns the device time in ms."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint32)
+        assert ids.size >= pos0 + n
+        ms = C.c_float(0)
+        _check(lib().nb200_batch_prefill(self.h, int(slot), _p(ids, u32p), int(pos0), int(n), C.byref(ms)))
+        return float(ms.value)
+
+    def next_greedy(self, slots, ids, pos, penalties) -> list:
+        """Entry i is Engine.next_greedy(ids[i], pos[i], 0, penalties[i]) in slot slots[i]; returns the next ids."""
+        n = len(slots)
+        assert len(ids) == len(pos) == len(penalties) == n
+        arrs = [np.ascontiguousarray(a, dtype=np.uint32) for a in ids]
+        ptrs = (u32p * n)(*[_p(a, u32p) for a in arrs])
+        s = np.asarray(slots, np.uint32); p = np.asarray(pos, np.uint32); pen = np.asarray(penalties, np.float32)
+        out = np.zeros(n, np.uint32)
+        ms = C.c_float(0)
+        _check(lib().nb200_batch_next_greedy(self.h, n, _p(s, u32p), ptrs, _p(p, u32p), _p(pen, f32p), _p(out, u32p), C.byref(ms)))
+        self.device_ms = float(ms.value)
+        return out.tolist()
+
+    def logits(self, slot: int) -> np.ndarray:
+        out = np.empty(self.engine.vocab, dtype=np.float32)
+        _check(lib().nb200_batch_read_logits(self.h, int(slot), _p(out, f32p)))
+        return out
+
+    def read(self, field: int, count: int, slot: int, layer: int = 0, pos: int = 0) -> np.ndarray:
+        """A K (F_KROW) or V (F_VROW) cache row of a slot, as Engine.read gives the engine's."""
+        out = np.zeros(count, dtype=np.float32)
+        _check(lib().nb200_batch_read_kv(self.h, int(slot), int(field), int(layer), int(pos), _p(out, f32p), int(count)))
+        return out
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().nb200_batch_destroy(self.h)
+            self.h = None
+            if self in self.engine._batches:
+                self.engine._batches.remove(self)
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None) and getattr(self.engine, "h", None):
+                self.close()
+        except Exception:
+            pass
 
 
 class TpGroup:
