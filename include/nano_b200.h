@@ -179,22 +179,36 @@ int nb200_prefill(nb200_engine *e, const uint32_t *ids, uint32_t pos0, uint32_t 
  *                            up as nb200_read_logits returns them after that call (penalised).  The entries run in passes of up
  *                            to M (info[0], at most 16) positions per pass over the weights.  device_ms (optional): CUDA-event
  *                            time of the call.
+ *   nb200_batch_next_sampled entry i with temperature[i] > 0 does what nb200_next_sampled(e, ids[i], pos[i], repetition_penalty[i],
+ *                            temperature[i], top_p[i], coin[i], &next_tokens[i], &top6[6 * i]) does, in slot slots[i]: the same
+ *                            penalised logits row, sampled id and six observed ids, and the same empty-nucleus rule (the
+ *                            first-max id, six zero ids).  An entry with temperature[i] == 0 is exactly nb200_batch_next_greedy's
+ *                            entry, with six zero ids, so greedy and sampled sessions share passes.  top6 (n x 6) is optional.
+ *                            Everything nb200_batch_next_greedy refuses is refused with the same message, and so is a negative or
+ *                            NaN temperature; top_p and coin are not checked, as for nb200_next_sampled.  The sampler's
+ *                            workspace is the batch's own, allocated at its first call with a sampled entry (a failed
+ *                            allocation fails the call before anything is written) and freed by nb200_batch_destroy; the
+ *                            engine's own sampler workspace is never used.  A sampled entry's result depends neither on the
+ *                            other entries of the call nor on which of them sample.
  *   nb200_batch_read_logits / nb200_batch_read_kv  a slot's logits row, and its K / V cache rows as nb200_read_buffer gives them.
  *   nb200_batch_info         [0] M, [1] n_slots, [2] the attention kernel (encoded as nb200_config.reserved[4]), [3] 0.
  * A batch always runs the multi-kernel path's arithmetic, and a row's value depends neither on the other entries of its pass nor
  * on how many there are: each slot's ids, logits and K / V rows are bit-identical to those of an engine created with the same
- * flags plus NB200_FLAG_NO_STREAM running that session alone (nb200_prefill + nb200_next_greedy) -- also when the batch's own
+ * flags plus NB200_FLAG_NO_STREAM running that session alone (nb200_prefill + nb200_next_greedy / nb200_next_sampled) -- also when the batch's own
  * engine runs the streaming kernel -- and in exact mode to the strict reference.  The engine's own cache, logits, seen set,
  * results and nb200_config.reserved[3..6] are not changed by a batch; its calls share the engine's stream.
  * NB200_EINVAL, with nothing written: a tensor-parallel engine or an active LoRA plug-in (checked at every call), n_slots == 0,
  * n == 0, a slot >= n_slots or the same slot twice in one call, a position >= min(max_seq_len, block_size), an id >= vocab_size.
- * Destroy every batch before its engine.  Not covered: temperature sampling, non-causal attention, LoRA, tensor parallelism. */
+ * Destroy every batch before its engine.  Not covered: non-causal attention, LoRA, tensor parallelism. */
 typedef struct nb200_batch nb200_batch;
 int nb200_batch_create(nb200_engine *e, uint32_t n_slots, nb200_batch **out);
 void nb200_batch_destroy(nb200_batch *b);
 int nb200_batch_prefill(nb200_batch *b, uint32_t slot, const uint32_t *ids, uint32_t pos0, uint32_t n, float *device_ms);
 int nb200_batch_next_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t *const *ids, const uint32_t *pos,
                             const float *repetition_penalty, uint32_t *next_tokens, float *device_ms);
+int nb200_batch_next_sampled(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t *const *ids, const uint32_t *pos,
+                             const float *repetition_penalty, const float *temperature, const float *top_p, const float *coin,
+                             uint32_t *next_tokens, uint32_t *top6 /* n x 6, optional */, float *device_ms);
 int nb200_batch_read_logits(nb200_batch *b, uint32_t slot, float *host_logits);
 int nb200_batch_read_kv(nb200_batch *b, uint32_t slot, int field /* NB200_F_KROW | NB200_F_VROW */, uint32_t layer, uint32_t pos,
                         float *dst, uint32_t count);

@@ -1525,11 +1525,17 @@ struct nb200_batch {
     std::vector<BatchPass> pass_host;         // [max_pass]
     uint32_t *ids_pass = nullptr, *ids_pass_host = nullptr;   // [n_slots] the ids the entries consume, the host copy pinned
     uint32_t *next_dev = nullptr, *next_host = nullptr;       // [n_slots] result ids, the host copy pinned
+    // sampling (nb200_batch_next_sampled), allocated at the first call with a sampled entry: the sampler's workspace for M rows,
+    // the per-entry result words {token, six ids, n0, first-max index} and their pinned host copy, the per-pass row tables
+    void *samp_ws = nullptr; size_t samp_cub = 0;
+    uint32_t *res_dev = nullptr, *res_host = nullptr;         // [n_slots][16]
+    std::vector<SampleRows> samp_pass;                        // [max_pass]
     LayerBufs buf;                            // M positions
     std::vector<std::vector<uint32_t>> mirror;
     std::vector<char> mirror_valid;
     std::vector<void *> allocs;
 };
+static_assert(kPrefillMax <= (int)kSampleRowsMax, "a pass's sampled entries fit one sampler launch");
 
 namespace {
 
@@ -1565,8 +1571,9 @@ int run_batch_matvec(nb200_engine *e, int epi, const Mat &mt, BatchMvArgs a) {
     return launch<BatchMvArgs>(e, k, dim3(grid), dim3(kThreads), smem, a);
 }
 
-// one pass: the m entries of bp (their ids also at ids on the device) -> their slots' K / V rows and logits, next ids at next[0..m)
-int run_batch_pass(nb200_batch *b, const BatchPass &bp, const uint32_t *ids, uint32_t m, uint32_t *next) {
+// one pass: the m entries of bp (their ids also at ids on the device) -> their slots' K / V rows and logits, next ids at next[0..m);
+// then the sampler over the pass's sampled entries sr (sr->n of them, none when sr is null), results at res[p * 16 ..]
+int run_batch_pass(nb200_batch *b, const BatchPass &bp, const uint32_t *ids, uint32_t m, uint32_t *next, const SampleRows *sr, uint32_t *res) {
     nb200_engine *e = b->e;
     const Dims &d = e->d;
     const LayerBufs &buf = b->buf;
@@ -1599,7 +1606,11 @@ int run_batch_pass(nb200_batch *b, const BatchPass &bp, const uint32_t *ids, uin
     a.bp = bp; a.logits = b->logits; a.seen = b->seen;
     if ((r = run_batch_matvec(e, EPI_CLS, e->cls, a))) return r;
     BatchArgmaxArgs am{b->logits, bp, next, d.V};
-    return launch<BatchArgmaxArgs>(e, k_batch_argmax, dim3(m), dim3(1024), 0, am);
+    if ((r = launch<BatchArgmaxArgs>(e, k_batch_argmax, dim3(m), dim3(1024), 0, am))) return r;
+    if (!sr || sr->n == 0) return 0;
+    CK(sample_rows_launch(b->samp_ws, b->samp_cub, b->M, b->logits, d.V, *sr, res, next, e->stream));
+    e->launches += 3;                 // prepare, sort, pick (counted as nb200_next_sampled counts its sampler)
+    return 0;
 }
 
 }  // namespace
@@ -1613,6 +1624,7 @@ void nb200_batch_destroy(nb200_batch *b) {
     for (void *p : b->allocs) cudaFree(p);
     if (b->ids_pass_host) cudaFreeHost(b->ids_pass_host);
     if (b->next_host) cudaFreeHost(b->next_host);
+    if (b->res_host) cudaFreeHost(b->res_host);
     delete b;
 }
 
@@ -1686,17 +1698,24 @@ int nb200_batch_prefill(nb200_batch *b, uint32_t slot, const uint32_t *ids, uint
     return 0;
 }
 
-int nb200_batch_next_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t *const *ids, const uint32_t *pos,
-                            const float *repetition_penalty, uint32_t *next_tokens, float *device_ms) {
+}  // extern "C"
+
+namespace {
+
+// nb200_batch_next_greedy (temperature null) and nb200_batch_next_sampled: every check, then one pass loop
+int batch_step(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t *const *ids, const uint32_t *pos, const float *repetition_penalty,
+               const float *temperature, const float *top_p, const float *coin, uint32_t *next_tokens, uint32_t *top6, float *device_ms) {
     int r;
     if ((r = batch_usable(b))) return r;
     nb200_engine *e = b->e;
     const Dims &d = e->d;
     if (!slots || !ids || !pos || !repetition_penalty || !next_tokens) return fail(NB200_EINVAL, "null argument");
+    if (temperature && (!top_p || !coin)) return fail(NB200_EINVAL, "null argument");
     if (n == 0) return fail(NB200_EINVAL, "no entries");
     // every check before anything is written
     std::vector<char> used(b->n_slots, 0);
     const uint32_t lim = pos_limit(d);
+    bool sampled = false;
     for (uint32_t i = 0; i < n; i++) {
         if (slots[i] >= b->n_slots) return fail(NB200_EINVAL, "entry %u: slot %u of a batch of %u", i, slots[i], b->n_slots);
         if (used[slots[i]]) return fail(NB200_EINVAL, "entry %u: slot %u appears twice in one call", i, slots[i]);
@@ -1706,17 +1725,38 @@ int nb200_batch_next_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, c
         const uint32_t upto = (repetition_penalty[i] != 1.0f) ? 0 : pos[i];      // the penalty reads ids[0..pos)
         for (uint32_t p = upto; p <= pos[i]; p++)
             if (ids[i][p] >= d.V) return fail(NB200_EINVAL, "entry %u: id %u at position %u out of range", i, ids[i][p], p);
+        if (temperature) {
+            if (!(temperature[i] >= 0.0f)) return fail(NB200_EINVAL, "entry %u: temperature %g is negative or NaN", i, (double)temperature[i]);
+            sampled |= temperature[i] != 0.0f;
+        }
     }
     CK(cudaSetDevice(e->device));
+    if (sampled && !b->samp_ws) {
+        void *ws = nullptr; uint32_t *res = nullptr;
+        size_t cub = 0;
+        const size_t bytes = sample_rows_workspace_bytes(d.V, b->M, &cub);
+        DMV(b->allocs, ws, bytes);
+        DMV(b->allocs, res, (size_t)b->n_slots * 16 * 4);
+        if (!b->res_host) CK(cudaHostAlloc(&b->res_host, (size_t)b->n_slots * 16 * 4, cudaHostAllocDefault));
+        b->samp_pass.resize(b->max_pass);
+        b->samp_ws = ws; b->samp_cub = cub; b->res_dev = res;
+    }
     struct Events { cudaEvent_t ev[2] = {nullptr, nullptr}; ~Events() { for (auto v : ev) if (v) cudaEventDestroy(v); } } evs;
     for (auto &v : evs.ev) CK(cudaEventCreate(&v));
     CK(cudaStreamSynchronize(e->stream));           // the pinned ids and results may still be in flight
     const uint32_t npass = (n + b->M - 1) / b->M;
+    for (uint32_t k = 0; sampled && k < npass; k++) b->samp_pass[k].n = 0;
     for (uint32_t i = 0; i < n; i++) {
         BatchPass &ps = b->pass_host[i / b->M];
         const uint32_t p = i % b->M;
         ps.slot[p] = slots[i]; ps.pos[p] = pos[i]; ps.pen[p] = repetition_penalty[i];
         b->ids_pass_host[i] = ids[i][pos[i]];
+        if (sampled && temperature[i] != 0.0f) {              // a sampled entry: the next row of its pass's sampler
+            SampleRows &sr = b->samp_pass[i / b->M];
+            sr.slot[sr.n] = slots[i]; sr.entry[sr.n] = p;
+            sr.temperature[sr.n] = temperature[i]; sr.top_p[sr.n] = top_p[i]; sr.coin[sr.n] = coin[i];
+            sr.n++;
+        }
     }
     CK(cudaEventRecord(evs.ev[0], e->stream));
     for (uint32_t i = 0; i < n; i++) {
@@ -1730,16 +1770,37 @@ int nb200_batch_next_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, c
     CK(cudaMemcpyAsync(b->ids_pass, b->ids_pass_host, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
     for (uint32_t k = 0; k < npass; k++) {
         const uint32_t m = (n - k * b->M < b->M) ? n - k * b->M : b->M;
-        if ((r = run_batch_pass(b, b->pass_host[k], b->ids_pass + k * b->M, m, b->next_dev + k * b->M))) return r;
+        if ((r = run_batch_pass(b, b->pass_host[k], b->ids_pass + k * b->M, m, b->next_dev + k * b->M, sampled ? &b->samp_pass[k] : nullptr,
+                                b->res_dev + (size_t)k * b->M * 16))) return r;
     }
     CK(cudaEventRecord(evs.ev[1], e->stream));
     CK(cudaMemcpyAsync(b->next_host, b->next_dev, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+    if (sampled && top6) CK(cudaMemcpyAsync(b->res_host, b->res_dev, (size_t)n * 16 * 4, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     memcpy(next_tokens, b->next_host, (size_t)n * 4);
+    if (top6)
+        for (uint32_t i = 0; i < n; i++)
+            for (uint32_t j = 0; j < 6; j++) top6[i * 6 + j] = (sampled && temperature[i] != 0.0f) ? b->res_host[i * 16 + 1 + j] : 0u;
     float ms = 0.0f;
     CK(cudaEventElapsedTime(&ms, evs.ev[0], evs.ev[1]));
     if (device_ms) *device_ms = ms;
     return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int nb200_batch_next_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t *const *ids, const uint32_t *pos,
+                            const float *repetition_penalty, uint32_t *next_tokens, float *device_ms) {
+    return batch_step(b, n, slots, ids, pos, repetition_penalty, nullptr, nullptr, nullptr, next_tokens, nullptr, device_ms);
+}
+
+int nb200_batch_next_sampled(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t *const *ids, const uint32_t *pos,
+                             const float *repetition_penalty, const float *temperature, const float *top_p, const float *coin,
+                             uint32_t *next_tokens, uint32_t *top6, float *device_ms) {
+    if (!temperature) return fail(NB200_EINVAL, "null argument");
+    return batch_step(b, n, slots, ids, pos, repetition_penalty, temperature, top_p, coin, next_tokens, top6, device_ms);
 }
 
 int nb200_batch_read_logits(nb200_batch *b, uint32_t slot, float *host_logits) {

@@ -20,14 +20,16 @@ namespace nb {
 constexpr int kSampThreads = 1024;
 constexpr int kSampChunk = 4096;       // floats staged in shared memory per step of a sequential scan
 
-// pass 1: y = logit / T, max; p = expf(y - max); sequential sum; p /= sum; key = p >= cutoff ? p : -1; out[7] = n0 = #candidates,
-// out[8] = the first index of the largest p
-__global__ void __launch_bounds__(kSampThreads) k_sample_prepare(const float *__restrict__ logits, uint32_t V, float temperature, float top_p,
-                                                                 float *keys, uint32_t *vals, uint32_t *out) {
+// pass 1 of one row: y = logit / T, max; p = expf(y - max); sequential sum; p /= sum; key = p >= cutoff ? p : -1, handed to
+// store(i, key) (scratch: V floats, read back before the store); out[7] = n0 = #candidates, out[8] = the first index of the largest p
+template <class Store>
+__device__ __forceinline__ void sample_prepare_row(const float *__restrict__ logits, uint32_t V, float temperature, float top_p, float *scratch,
+                                                   Store store, uint32_t *out) {
     __shared__ float red[32];
     __shared__ float chunk[kSampChunk];
     __shared__ float s_total;
     __shared__ uint32_t s_cnt, s_best[32];
+    float *keys = scratch;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float mx = -FLT_MAX;
     for (uint32_t i = threadIdx.x; i < V; i += kSampThreads) {
@@ -60,8 +62,7 @@ __global__ void __launch_bounds__(kSampThreads) k_sample_prepare(const float *__
     for (uint32_t i = threadIdx.x; i < V; i += kSampThreads) {
         const float p = __fdiv_rn(keys[i], total);                   // infer.c:632
         const bool in = p >= cutoff;
-        keys[i] = in ? p : -1.0f;
-        vals[i] = i;
+        store(i, in ? p : -1.0f);
         cnt += in ? 1u : 0u;
         if (p > bp) { bp = p; bi = i; }                              // ascending i per thread: the thread's first max
     }
@@ -82,9 +83,16 @@ __global__ void __launch_bounds__(kSampThreads) k_sample_prepare(const float *__
     }
 }
 
-// pass 2 (after the sort): cumulative sum to top_p, then the CDF walk (infer.c:1076-1106), both sequential
-__global__ void __launch_bounds__(256) k_sample_pick(const float *__restrict__ keys, const uint32_t *__restrict__ vals, float top_p, float coin,
-                                                     uint32_t *out, DevState *st) {
+__global__ void __launch_bounds__(kSampThreads) k_sample_prepare(const float *__restrict__ logits, uint32_t V, float temperature, float top_p,
+                                                                 float *keys, uint32_t *vals, uint32_t *out) {
+    sample_prepare_row(logits, V, temperature, top_p, keys, [&](uint32_t i, float key) { keys[i] = key; vals[i] = i; }, out);
+}
+
+// pass 2 of one row (after the sort; key(i) = the i-th largest key, vals the vocabulary indices in that order): cumulative sum
+// to top_p, then the CDF walk (infer.c:1076-1106), both sequential.  Thread 0 writes out[0..6] = {token, six ids} and calls
+// done(token).
+template <class Key, class Done>
+__device__ __forceinline__ void sample_pick_row(Key key, const uint32_t *__restrict__ vals, float top_p, float coin, uint32_t *out, Done done) {
     __shared__ float chunk[kSampChunk];
     __shared__ uint32_t s_stop, s_last;
     __shared__ float s_cum;
@@ -96,7 +104,7 @@ __global__ void __launch_bounds__(256) k_sample_pick(const float *__restrict__ k
             const uint32_t tok = out[8];
             out[0] = tok;
             for (uint32_t i = 0; i < 6; i++) out[1 + i] = 0u;
-            if (st) st->next_token = tok;
+            done(tok);
         }
         return;
     }
@@ -105,7 +113,7 @@ __global__ void __launch_bounds__(256) k_sample_pick(const float *__restrict__ k
     float cum = 0.0f;
     for (uint32_t c0 = 0; c0 < n0 && !s_stop; c0 += kSampChunk) {
         const uint32_t n = min((uint32_t)kSampChunk, n0 - c0);
-        for (uint32_t i = threadIdx.x; i < n; i += 256) chunk[i] = keys[c0 + i];
+        for (uint32_t i = threadIdx.x; i < n; i += 256) chunk[i] = key(c0 + i);
         __syncthreads();
         if (threadIdx.x == 0) {
             for (uint32_t i = 0; i < n; i++) {
@@ -125,7 +133,7 @@ __global__ void __launch_bounds__(256) k_sample_pick(const float *__restrict__ k
     uint32_t pick = last;
     for (uint32_t c0 = 0; c0 <= last && !s_stop; c0 += kSampChunk) {
         const uint32_t n = min((uint32_t)kSampChunk, last + 1 - c0);
-        for (uint32_t i = threadIdx.x; i < n; i += 256) chunk[i] = keys[c0 + i];
+        for (uint32_t i = threadIdx.x; i < n; i += 256) chunk[i] = key(c0 + i);
         __syncthreads();
         if (threadIdx.x == 0) {
             for (uint32_t i = 0; i < n; i++) {
@@ -140,8 +148,13 @@ __global__ void __launch_bounds__(256) k_sample_pick(const float *__restrict__ k
         const uint32_t tok = vals[s_stop ? s_last : last];
         out[0] = tok;
         for (uint32_t i = 0; i < 6; i++) out[1 + i] = (n0 > i) ? vals[i] : 0u;        // the observation hook's token_0..5 (infer.c:1086-1096)
-        if (st) st->next_token = tok;
+        done(tok);
     }
+}
+
+__global__ void __launch_bounds__(256) k_sample_pick(const float *__restrict__ keys, const uint32_t *__restrict__ vals, float top_p, float coin,
+                                                     uint32_t *out, DevState *st) {
+    sample_pick_row([&](uint32_t i) { return keys[i]; }, vals, top_p, coin, out, [&](uint32_t tok) { if (st) st->next_token = tok; });
 }
 
 // The workspace: keys and values in and out (V words each, 256-byte aligned), the sort's temporary storage, then the result
@@ -179,6 +192,97 @@ cudaError_t sample_top_p_launch(void *workspace, size_t cub_bytes, const float *
     if (e != cudaSuccess) return e;
     k_sample_pick<<<1, 256, 0, stream>>>(w.keys_out, w.vals_out, top_p, coin, w.out, st);
     *out_dev = w.out;
+    return cudaGetLastError();
+}
+
+// ---------------- several rows per launch (nb200_batch_next_sampled) ----------------
+// One prepare CTA and one pick CTA per row, each running the single-row arithmetic above on its own row, and one stable
+// device-wide radix sort over all rows: row j's key is ((n - 1 - j) << 32) | key_bits(p), so a descending sort keeps the rows
+// apart in row order and orders each row exactly as the single-row sort does (keys are -1 or finite p >= +0, whose float order
+// is key_bits' unsigned order; equal keys keep index order).
+__host__ __device__ __forceinline__ uint32_t key_bits(float p) {
+#ifdef __CUDA_ARCH__
+    const uint32_t u = __float_as_uint(p);
+#else
+    uint32_t u; memcpy(&u, &p, 4);
+#endif
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__host__ __device__ __forceinline__ float key_float(uint32_t b) {
+    const uint32_t u = (b & 0x80000000u) ? (b & 0x7fffffffu) : ~b;
+#ifdef __CUDA_ARCH__
+    return __uint_as_float(u);
+#else
+    float p; memcpy(&p, &u, 4); return p;
+#endif
+}
+
+// rows sized for `rows` rows: composite keys in and out, values in and out (rows * V words each, 256-byte aligned), the sort's
+// temporary storage.  Row j's float scratch of the prepare pass is keys_out + j * V read as floats (dead before the sort).
+struct SampleRowsWorkspace {
+    unsigned long long *keys_in, *keys_out;
+    uint32_t *vals_in, *vals_out;
+    void *tmp;
+};
+
+static inline SampleRowsWorkspace sample_rows_workspace(void *workspace, uint32_t V, uint32_t rows) {
+    const size_t n = (size_t)V * rows, a8 = (n * 8 + 255) & ~(size_t)255, a4 = (n * 4 + 255) & ~(size_t)255;
+    unsigned char *w = static_cast<unsigned char *>(workspace);
+    return {reinterpret_cast<unsigned long long *>(w), reinterpret_cast<unsigned long long *>(w + a8), reinterpret_cast<uint32_t *>(w + 2 * a8),
+            reinterpret_cast<uint32_t *>(w + 2 * a8 + a4), w + 2 * a8 + 2 * a4};
+}
+
+size_t sample_rows_workspace_bytes(uint32_t V, uint32_t rows, size_t *cub_bytes) {
+    const size_t n = (size_t)V * rows;
+    size_t tmp = 0;
+    cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
+                                              (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)n, 0, 64);
+    if (cub_bytes) *cub_bytes = tmp;
+    return 2 * ((n * 8 + 255) & ~(size_t)255) + 2 * ((n * 4 + 255) & ~(size_t)255) + tmp;
+}
+
+struct SampleRowsArgs {
+    SampleRows r;                     // by value: each CTA reads its row's parameters from the parameter bank
+    const float *logits;              // [slots][V]
+    uint32_t V;
+    SampleRowsWorkspace w;
+    uint32_t *res, *next;             // res[entry * 16 ..]: {token, six ids, n0, first-max index}; next[entry] = token
+};
+
+__global__ void __launch_bounds__(kSampThreads) k_sample_rows_prepare(const SampleRowsArgs a) {
+    const uint32_t j = blockIdx.x, V = a.V;
+    const size_t off = (size_t)j * V;
+    unsigned long long *keys = a.w.keys_in + off;
+    uint32_t *vals = a.w.vals_in + off;
+    const unsigned long long row = (unsigned long long)(a.r.n - 1 - j) << 32;
+    sample_prepare_row(a.logits + (size_t)a.r.slot[j] * V, V, a.r.temperature[j], a.r.top_p[j], reinterpret_cast<float *>(a.w.keys_out) + off,
+                       [&](uint32_t i, float key) { keys[i] = row | key_bits(key); vals[i] = i; }, a.res + (size_t)a.r.entry[j] * 16);
+}
+
+__global__ void __launch_bounds__(256) k_sample_rows_pick(const SampleRowsArgs a) {
+    const uint32_t j = blockIdx.x;
+    const size_t off = (size_t)j * a.V;
+    const unsigned long long *keys = a.w.keys_out + off;
+    const uint32_t entry = a.r.entry[j];
+    uint32_t *next = a.next;
+    sample_pick_row([&](uint32_t i) { return key_float((uint32_t)keys[i]); }, a.w.vals_out + off, a.r.top_p[j], a.r.coin[j],
+                    a.res + (size_t)entry * 16, [&](uint32_t tok) { next[entry] = tok; });
+}
+
+cudaError_t sample_rows_launch(void *workspace, size_t cub_bytes, uint32_t rows, const float *logits, uint32_t V, const SampleRows &r,
+                               uint32_t *res, uint32_t *next, cudaStream_t stream) {
+    if (r.n == 0 || r.n > rows || r.n > kSampleRowsMax) return cudaErrorInvalidValue;
+    const SampleRowsArgs a{r, logits, V, sample_rows_workspace(workspace, V, rows), res, next};
+    k_sample_rows_prepare<<<r.n, kSampThreads, 0, stream>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    int end_bit = 32;                 // the row field needs ceil(log2 n) bits above the probability's 32
+    while ((1u << (end_bit - 32)) < r.n) end_bit++;
+    size_t tb = cub_bytes;
+    e = cub::DeviceRadixSort::SortPairsDescending(a.w.tmp, tb, a.w.keys_in, a.w.keys_out, a.w.vals_in, a.w.vals_out, (int)((size_t)r.n * V), 0,
+                                                  end_bit, stream);
+    if (e != cudaSuccess) return e;
+    k_sample_rows_pick<<<r.n, 256, 0, stream>>>(a);
     return cudaGetLastError();
 }
 

@@ -32,8 +32,8 @@ EXPORTS = [
     "nb200_op_q4k_quantize_blocks", "nb200_op_q4k_matvec_blocks",
     "nb200_lora_load", "nb200_lora_enable", "nb200_lora_unload",
     "nb200_engine_create_tp", "nb200_tp_export", "nb200_tp_attach_ipc", "nb200_tp_attach_local",
-    "nb200_batch_create", "nb200_batch_destroy", "nb200_batch_prefill", "nb200_batch_next_greedy", "nb200_batch_read_logits",
-    "nb200_batch_read_kv", "nb200_batch_info",
+    "nb200_batch_create", "nb200_batch_destroy", "nb200_batch_prefill", "nb200_batch_next_greedy", "nb200_batch_next_sampled",
+    "nb200_batch_read_logits", "nb200_batch_read_kv", "nb200_batch_info",
 ]
 
 
@@ -100,6 +100,8 @@ def lib():
         L.nb200_batch_destroy.argtypes = [C.c_void_p]
         L.nb200_batch_prefill.argtypes = [C.c_void_p, C.c_uint32, u32p, C.c_uint32, C.c_uint32, f32p]
         L.nb200_batch_next_greedy.argtypes = [C.c_void_p, C.c_uint32, u32p, C.POINTER(u32p), u32p, f32p, u32p, f32p]
+        L.nb200_batch_next_sampled.argtypes = [C.c_void_p, C.c_uint32, u32p, C.POINTER(u32p), u32p, f32p, f32p, f32p, f32p, u32p, u32p,
+                                               f32p]
         L.nb200_batch_read_logits.argtypes = [C.c_void_p, C.c_uint32, f32p]
         L.nb200_batch_read_kv.argtypes = [C.c_void_p, C.c_uint32, C.c_int, C.c_uint32, C.c_uint32, f32p, C.c_uint32]
         L.nb200_batch_info.argtypes = [C.c_void_p, u32p]
@@ -320,7 +322,7 @@ class Batch:
         self.engine = engine
         self.h = C.c_void_p()
         _check(lib().nb200_batch_create(engine.h, int(n_slots), C.byref(self.h)))
-        self.device_ms = 0.0        # device time of the last next_greedy
+        self.device_ms = 0.0        # device time of the last next_greedy / next_sampled
 
     def info(self) -> dict:
         """{"chunk": positions per pass M, "slots": n_slots, "attention": the attention kernel, named as Engine.kernels()}"""
@@ -348,6 +350,22 @@ class Batch:
         _check(lib().nb200_batch_next_greedy(self.h, n, _p(s, u32p), ptrs, _p(p, u32p), _p(pen, f32p), _p(out, u32p), C.byref(ms)))
         self.device_ms = float(ms.value)
         return out.tolist()
+
+    def next_sampled(self, slots, ids, pos, penalties, temperatures, top_ps, coins):
+        """Entry i is Engine.next_sampled(ids[i], pos[i], penalties[i], temperatures[i], top_ps[i], coins[i]) in slot slots[i],
+        or next_greedy's entry where temperatures[i] == 0 (its six ids are zeros); returns (next ids, six ids per entry)."""
+        n = len(slots)
+        assert len(ids) == len(pos) == len(penalties) == len(temperatures) == len(top_ps) == len(coins) == n
+        arrs = [np.ascontiguousarray(a, dtype=np.uint32) for a in ids]
+        ptrs = (u32p * n)(*[_p(a, u32p) for a in arrs])
+        s = np.asarray(slots, np.uint32); p = np.asarray(pos, np.uint32)
+        pen, T, tp, c = (np.asarray(v, np.float32) for v in (penalties, temperatures, top_ps, coins))
+        out = np.zeros(n, np.uint32); six = np.zeros((n, 6), np.uint32)
+        ms = C.c_float(0)
+        _check(lib().nb200_batch_next_sampled(self.h, n, _p(s, u32p), ptrs, _p(p, u32p), _p(pen, f32p), _p(T, f32p), _p(tp, f32p),
+                                              _p(c, f32p), _p(out, u32p), _p(six, u32p), C.byref(ms)))
+        self.device_ms = float(ms.value)
+        return out.tolist(), six.tolist()
 
     def logits(self, slot: int) -> np.ndarray:
         out = np.empty(self.engine.vocab, dtype=np.float32)
