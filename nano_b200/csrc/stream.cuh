@@ -78,6 +78,20 @@ __device__ __forceinline__ uint32_t st_tid() { uint32_t t; asm volatile("mov.u32
 // barrier among the 15 consumer warps only (the producer warp never takes part)
 __device__ __forceinline__ void cbar() { asm volatile("bar.sync 1, %0;" ::"n"(kConsThreads) : "memory"); }
 
+// Per-group ready marks of an activation operand whose groups are quantised one at a time (st_prep on a phase without
+// rmsnorm): mark j holds the epoch of the exchange whose group j the operand's codes and scale now hold.  The owning
+// warp stores it with release order after its lanes' code stores; a consumer warp acquires the marks before its row dots.
+// The marks are passed around as 32-bit shared-memory addresses (0: the operand has no marks): a generic pointer would take
+// two of the consumers' registers through every row loop.
+__device__ __forceinline__ void st_mark_ready(uint32_t f, uint32_t epoch) {
+    asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(f), "r"(epoch) : "memory");
+}
+__device__ __forceinline__ uint32_t st_ld_ready(uint32_t f) {
+    uint32_t v;
+    asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(f) : "memory");
+    return v;
+}
+
 // ---------------------------------------------------------------- exchange words {value, epoch}
 __device__ __forceinline__ void xw_ld2(const unsigned long long *p, unsigned long long &a, unsigned long long &b) {
     asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "l"(p) : "memory");
@@ -121,6 +135,36 @@ __device__ __forceinline__ float xw_poll1(const unsigned long long *p, uint32_t 
         } while (!xw_ok(a, need));
     }
     return xw_val(a);
+}
+// A whole warp waits until marks 0..G-1 all hold `need` (lane l looks at marks l, l + 32, ...).  The loops are warp-uniform:
+// a spin that lanes leave one by one needs a convergence barrier, and with the consumers at the 128-register cap the extra
+// barrier state went to local memory.
+__device__ __forceinline__ void st_wait_ready_warp(uint32_t f, uint32_t G, uint32_t need, uint32_t *err) {
+    const uint32_t lane = st_tid() & 31u;
+    long long t0 = 0;
+    for (uint32_t it = 1;; it++) {
+        bool ok = true;
+        for (uint32_t j0 = 0; j0 < G; j0 += 32u) {
+            const uint32_t m = j0 + lane < G ? st_ld_ready(f + 4u * (j0 + lane)) : need;
+            ok = ok && (m == need || m == kXwAny);          // kXwAny: NB200_ABLATE & 16 (the prologue took any epoch)
+        }
+        if (__all_sync(0xffffffffu, ok)) break;
+        __nanosleep(20);          // the owning warps are quantising: leave them the MIO pipe (see mbar_wait)
+        xw_spin_guard(it, t0, err, 0x52u);
+    }
+}
+// xw_poll4 for a whole warp (lanes with `on` false take part and read 0.0f): it leaves the loop once every lane's words carry
+// `need` (warp-uniform, for the reason given at st_wait_ready_warp)
+__device__ __forceinline__ float4 xw_poll4_warp(const unsigned long long *p, bool on, uint32_t need, uint32_t *err, uint32_t code) {
+    unsigned long long a = 0ull, b = 0ull, c = 0ull, d = 0ull;
+    long long t0 = 0;
+    for (uint32_t it = 1;; it++) {
+        if (on) { xw_ld2(p, a, b); xw_ld2(p + 2, c, d); }
+        const bool ok = !on || (xw_ok(a, need) && xw_ok(b, need) && xw_ok(c, need) && xw_ok(d, need));
+        if (__all_sync(0xffffffffu, ok)) break;
+        xw_spin_guard(it, t0, err, code);
+    }
+    return make_float4(xw_val(a), xw_val(b), xw_val(c), xw_val(d));
 }
 // one element into every replica of a vector, the stores spread over the `ts` lanes of a team (tl = lane within the team)
 __device__ __forceinline__ void xw_publish(unsigned long long *base, uint32_t rs, uint32_t idx, float v, uint32_t epoch, uint32_t tl, uint32_t ts) {
@@ -244,10 +288,18 @@ static __device__ void st_producer(const StreamArgs &g, const StRing &r, const S
 #endif
 constexpr int kStPollB = 2;          // Q80 / F32 warp slots whose exchange words are polled together
 static_assert(kStKmax % kStPollB == 0, "stream kernel: poll batches cover the warp slots");
-template <int QUANT, int LPG>
+// PG (Q80 / Q4K phases without a gain, i.e. O and W2; a source of exchange words): a group's codes depend on that group's
+// elements only, so every warp polls, quantises and marks its own groups (word j at shared address `ready` + 4j = need) one
+// at a time, and there is no closing barrier -- each warp waits for the marks before its row dots (st_consume).
+// Otherwise the prologue ends with a barrier.  (A separate instantiation: its registers are allocated apart from the
+// normalised prologue's.)
+template <int QUANT, int LPG, bool PG = false>
 __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long long *xsrc, const float *ssrc, uint32_t need, const float *__restrict__ gain,
-                                        uint32_t n, unsigned char *act, float *red, unsigned long long *dbg) {
+                                        uint32_t n, unsigned char *act, float *red, unsigned long long *dbg, uint32_t ready = 0u) {
     const int lane = st_tid() & 31, warp = st_tid() >> 5;
+    constexpr bool pg = PG;
+    static_assert(!PG || QUANT != 0x00, "stream kernel: F32 operands are not handed over per group");
+    if constexpr (PG) { gain = nullptr; ssrc = nullptr; }
     ST_DBG(0);
     if (gain) {      // the gain is applied after the sum of squares: start pulling its lines into L1 while the source is awaited
         for (uint32_t i = st_tid() * 32u; i < n; i += kConsThreads * 32u) asm volatile("prefetch.global.L1 [%0];" ::"l"(gain + i));
@@ -281,8 +333,8 @@ __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long
 #pragma unroll
             for (int h = 0; h < 2; h++) {
                 v[j][h] = make_float4(0, 0, 0, 0);
-                if (b < NB) {
-                    v[j][h] = ssrc ? *reinterpret_cast<const float4 *>(ssrc + base + 4 * h) : xw_poll4(xsrc + base + 4 * h, need, g.err);
+                if (b < NB && !pg) {
+                    v[j][h] = ssrc ? *reinterpret_cast<const float4 *>(ssrc + base + 4 * h) : xw_poll4_warp(xsrc + base + 4 * h, true, need, g.err, 0x50u);
                     ss = sq(v[j][h], ss);
                 }
             }
@@ -291,11 +343,18 @@ __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long
         float inv = 1.0f;
         if (gain) inv = inverse(ss);
         ST_DBG(2);
-#pragma unroll
+        // (PG: a rolled loop -- its state is one block's values, and the unrolled copies pushed the kernel past its registers)
+#pragma unroll (PG ? 1 : kStKmaxQ4K)
         for (int j = 0; j < kStKmaxQ4K; j++) {
             const uint32_t b = warp + kConsWarps * j;
             if (b < NB) {                                            // warp-uniform
-                float4 a0 = v[j][0], a1 = v[j][1];
+                float4 a0, a1;
+                if constexpr (PG) {
+                    a0 = xw_poll4_warp(xsrc + b * 256u + lane * 8u, true, need, g.err, 0x53u);
+                    a1 = xw_poll4_warp(xsrc + b * 256u + lane * 8u + 4u, true, need, g.err, 0x53u);
+                } else {
+                    a0 = v[j][0]; a1 = v[j][1];
+                }
                 if (gain) {
                     const float4 *gp4 = reinterpret_cast<const float4 *>(gain + b * 256u + lane * 8u);
                     a0 = nrm(a0, __ldg(gp4), inv); a1 = nrm(a1, __ldg(gp4 + 1), inv);
@@ -306,6 +365,7 @@ __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long
                 xe[b * 32 + lane] = c[0] | (c[2] << 8) | (c[4] << 16) | (c[6] << 24);
                 xo[b * 32 + lane] = c[1] | (c[3] << 8) | (c[5] << 16) | (c[7] << 24);
                 if ((lane & 3) == 0) gp[b * 8 + (lane >> 2)] = make_float4(__fmul_rn((float)s6, sc), __fmul_rn((float)b6, sbias), (float)csum, 0.0f);
+                if (pg) { __syncwarp(); if (lane == 0) st_mark_ready(ready + 4u * b, need); }
             }
         }
     } else {
@@ -338,10 +398,11 @@ __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long
         // Qwen3-0.6B) is one batch, i.e. one round trip.  Only the first batch stays in registers until the quantise pass;
         // later batches are read again there (their words cannot change before this CTA has published its next exchange).
         // Holding all six slots took 48 staging + 24 value registers and spilled to local memory on every phase.
+        // Per group (PG): no batches -- each slot is polled just before it is quantised.
         float4 v[kStPollB];
         float ss = 0.0f;
 #pragma unroll
-        for (int j0 = 0; j0 < kStKmax; j0 += kStPollB) {
+        for (int j0 = 0; j0 < (pg ? 0 : kStKmax); j0 += kStPollB) {
             float4 vb[kStPollB];
             if (ssrc) {
 #pragma unroll
@@ -379,13 +440,15 @@ __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long
         float inv = 1.0f;
         if (gain && !(g.ablate & 8u)) inv = inverse(ss);
         ST_DBG(2);
-#pragma unroll
+#pragma unroll (PG ? 1 : kStKmax)
         for (int j = 0; j < kStKmax; j++) {
             const uint32_t g0 = (warp + kConsWarps * j) * GW;
             if (g0 < G) {                                            // warp-uniform
                 const uint32_t gi = g0 + sub, i = gi * gs + li * 4u;
                 const bool on = i < n;
-                float4 a = (j < kStPollB) ? v[j] : reread(j);
+                float4 a;
+                if constexpr (PG) a = xw_poll4_warp(xsrc + (on ? i : 0u), on, need, g.err, 0x53u);
+                else a = (j < kStPollB) ? v[j] : reread(j);
                 if (gain && on) a = nrm(a, __ldg(reinterpret_cast<const float4 *>(gain + i)), inv);
                 if constexpr (QUANT == 0x00) {
                     if (on) *reinterpret_cast<float4 *>(act + (size_t)i * 4u) = a;
@@ -429,12 +492,13 @@ __device__ __forceinline__ void st_prep(const StreamArgs &g, const unsigned long
                         *reinterpret_cast<uint32_t *>(codes + i) = pk;
                         if (li == 0) scales[gi] = sc;
                     }
+                    if (pg) { __syncwarp(gmask); if (li == 0 && gi < G) st_mark_ready(ready + 4u * gi, need); }
                 }
             }
         }
     }
     ST_DBG(3);
-    cbar();
+    if (!pg) cbar();
     ST_DBG(4);
 }
 
@@ -576,9 +640,14 @@ __device__ __forceinline__ float st_row_q4k(const unsigned char *wrow, const uns
 template <int QUANT, int LPG>
 __device__ __forceinline__ void st_consume(const StreamArgs &g, const StRing &r, StCursor &c, uint32_t &tcount, const StKind &k, uint32_t epi, uint32_t layer,
                                            uint32_t row0, uint32_t rows, uint32_t epoch, const unsigned char *act, uint32_t pos, float pen,
-                                           float *xown, MatvecSmem &ms, const StGeo &geo, uint32_t kid, unsigned long long *dbg) {
+                                           float *xown, MatvecSmem &ms, const StGeo &geo, uint32_t kid, uint32_t ready,
+                                           unsigned long long *dbg) {
     const Dims &d = g.d;
     const int lane = st_tid() & 31, warp = st_tid() >> 5;
+    // `ready`: the operand's groups carry per-group marks (st_prep) of the source's epoch, the one before `epoch`.  A warp
+    // starts its rows once the groups are all in place; it waits on the marks, not on a barrier with the other warps, so it
+    // waits for the data it reads and nothing else (the row dots and their fp32 sums are as without marks).
+    if (ready) st_wait_ready_warp(ready, QUANT == 0x42 ? k.n / 256u : k.n / (LPG * 16u), epoch - 1u, g.err);
     float bestv = -FLT_MAX; uint32_t besti = 0xffffffffu;
     // epilogue of one finished row (value in all `ts` lanes of its team; `ri` = index among the rows this CTA owns)
     auto emit = [&](uint32_t row, uint32_t ri, float v, float v3, bool pub, uint32_t tl, uint32_t ts) {
@@ -1028,6 +1097,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
     __shared__ float xown[kStOwnMax];
     __shared__ volatile uint32_t s_progress;
     __shared__ unsigned int s_target;
+    __shared__ uint32_t s_ready[2][kStGroupsMax];        // per-group ready marks of the two activation operands (epoch 0: never handed out)
     __shared__ StStep ss;
     const Dims &d = g.d;
     const uint32_t cta = blockIdx.x, ncta = gridDim.x;
@@ -1046,6 +1116,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
         ss.tok = __ldcg(&g.st->use_token) ? __ldcg(&g.st->token) : __ldcg(g.ids + ss.pos);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+    for (uint32_t i = threadIdx.x; i < 2u * kStGroupsMax; i += kThreads) s_ready[i / kStGroupsMax][i % kStGroupsMax] = 0u;
     if (threadIdx.x < 5) {          // the rows this CTA owns of every kind (64-bit divisions: once, not once per phase)
         const StKind &k = g.kind[threadIdx.x];
         const uint32_t u0 = (uint32_t)(((uint64_t)cta * k.units) / ncta), u1 = (uint32_t)(((uint64_t)(cta + 1) * k.units) / ncta);
@@ -1132,9 +1203,22 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
                 if (own.rows[kid]) {          // CTA-uniform: a CTA without rows of this kind neither reads the source nor publishes
                     act_flip ^= 1u;
                     unsigned char *act = ssm + (act_flip ? g.off_act2 : g.off_act);
-                    st_prep<QUANT, LPG>(g, xsrc, ssrc, need, gain, k.n, act, ms.red, dbg);
+                    // O and W2 (no rmsnorm): the operand is quantised and handed to the row dots one group at a time
+                    // (decided from the loop counters only, which the compiler sees are warp-uniform).  A prologue writes the operand
+                    // (and marks) that the phase two prologues back read, and such a prologue has no closing barrier: the
+                    // prologue of the phase before it (QKV, W1|W3: rmsnorm) keeps every warp's reads of the older phase, and
+                    // its residual rows, before the writes.  A CTA that owns no rows of that phase takes a barrier instead.
+                    const bool pg = QUANT != 0x00 && !cls && (ph == SK_O || ph == SK_W2);
+                    const uint32_t ready = pg ? smem_u32(s_ready[act_flip]) : 0u;
+                    if (pg && own.rows[kid - 1u] == 0u) cbar();
+                    if constexpr (QUANT != 0x00) {
+                        if (pg) st_prep<QUANT, LPG, true>(g, xsrc, ssrc, need, gain, k.n, act, ms.red, dbg, ready);
+                        else st_prep<QUANT, LPG>(g, xsrc, ssrc, need, gain, k.n, act, ms.red, dbg);
+                    } else {
+                        st_prep<QUANT, LPG>(g, xsrc, ssrc, need, gain, k.n, act, ms.red, dbg);
+                    }
                     ST_STAMP();
-                    st_consume<QUANT, LPG>(g, ring_of(), cur, tcount, k, epi, l, own.row0[kid], own.rows[kid], eout, act, ss.pos, ss.pen, xown, ms, geo, kid, dbg);
+                    st_consume<QUANT, LPG>(g, ring_of(), cur, tcount, k, epi, l, own.row0[kid], own.rows[kid], eout, act, ss.pos, ss.pen, xown, ms, geo, kid, ready, dbg);
                 } else {
                     ST_STAMP();
                     const uint32_t t = st_tid();

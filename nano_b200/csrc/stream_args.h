@@ -58,6 +58,8 @@ __host__ __device__ inline uint32_t st_prep_max_n(uint32_t quant, uint32_t gs) {
     (void)gs;
     return quant == 0x42u ? (uint32_t)kConsWarps * kStKmaxQ4K * 256u : (uint32_t)kConsWarps * kStKmax * 128u;
 }
+// quantisation groups (Q80, 64 elements at least) or blocks (Q4K) of an operand of at most st_prep_max_n elements
+constexpr int kStGroupsMax = kConsWarps * kStKmax * 128 / 64;
 
 // attention workspace of one CTA (floats): q [KVM][hd] | scores of a segment [KVM][seg rows] | per-head scale [KVM] |
 // the position's k, v [2][hd] | the item's partial [KVM][hd + 2]; the merge of a multi-split head stages the partials of
