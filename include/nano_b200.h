@@ -70,8 +70,8 @@ typedef struct nb200_config {
                                    epilogues store 0, qkv 1, residual 2, swiglu 3, classifier 4 (the exact-mode F32 kernel sets none);
                                [4] attention kernel of the last layer run: 0 none yet, 1 exact, 2 generic split-KV,
                                    3 | kv_mul << 8 the split-KV kernel specialised for that kv_mul;
-                               nb200_prefill: [5] positions per chunk M (0 until the first call), [6] the attention kernel of the
-                                   last prefill, encoded as [4] */
+                               nb200_prefill and nb200_verify_greedy: [5] positions per chunk M (0 until the first call), [6] the
+                                   attention kernel of the last prefill or verify pass, encoded as [4] */
 } nb200_config;
 
 /* fields readable with nb200_read_buffer (same numbering as oracle probes) */
@@ -168,6 +168,45 @@ int nb200_decode_greedy(nb200_engine *e, uint32_t *ids, uint32_t n_prompt, uint3
  * Not covered: the streaming kernel's own prompt loop (nb200_decode_greedy and the shim keep running the prompt token by token,
  * so their fast-mode K/V bits do not change), tensor cores, non-causal (seq2seq) attention. */
 int nb200_prefill(nb200_engine *e, const uint32_t *ids, uint32_t pos0, uint32_t n, float *device_ms);
+
+/* Speculative greedy decoding (no reference counterpart), lossless: the ids are exactly those of nb200_next_greedy.
+ *   nb200_verify_greedy  ids[0..pos] are known (ids[pos] is consumed, as for nb200_next_greedy) and ids[pos+1 .. pos+n) are n-1
+ *                        drafted ids.  One pass over the weights runs positions pos .. pos+n-1 as a prefill chunk and the
+ *                        batch's classifier and argmax on each, so g_j, the greedy id at pos+j, is exactly what
+ *                        nb200_next_greedy(e, ids, pos+j, 0, repetition_penalty) returns on an engine created with the same flags
+ *                        plus NB200_FLAG_NO_STREAM (its penalty reads ids[0..pos+j), drafts included).  *n_accepted = a, the
+ *                        largest count with g_j == ids[pos+j+1] for every j < a; ids[pos+a+1] = g_a (the correction, or the
+ *                        bonus id when every draft is accepted), so ids needs pos+n+1 entries; ids past pos+a+1 keep the
+ *                        rejected drafts.  Afterwards the engine is where nb200_next_greedy at pos .. pos+a leaves it: K/V rows
+ *                        pos .. pos+a written, rows from pos+a+1 on as they were before the call (the rows the pass wrote there
+ *                        are saved first and restored), nb200_read_logits gives the penalised logits at pos+a, and the next
+ *                        nb200_next_greedy / nb200_next_sampled at pos+a+1 gives the same bits, on either execution path.
+ *                        Launches: the chunk's 1 + 6 * n_layer, the classifier, the argmax; when repetition_penalty != 1 also
+ *                        one seen-row kernel, and nb200_next_greedy's seen-set update when ids[0..pos) has new ids.  One host
+ *                        synchronise.  nb200_config.reserved[5] / [6] report M and the
+ *                        attention kernel after a call, as after nb200_prefill.  device_ms (optional): CUDA-event time of the pass.
+ *                        The workspace (M logits rows, M seen rows, the saved K/V rows) is allocated at the first call.
+ *                        NB200_EINVAL, with nothing written (cache, logits, seen set, ids): n == 0 or n > M (the chunk size),
+ *                        pos + n > min(max_seq_len, block_size), an id >= vocab_size in ids[pos .. pos+n) (and in ids[0..pos)
+ *                        when repetition_penalty != 1), a tensor-parallel engine, an active LoRA plug-in.
+ *   nb200_decode_lookup  nb200_decode_greedy's arguments and limits, with drafts looked up in the context itself (prompt lookup):
+ *                        its ids are bit-identical to nb200_decode_greedy's on an engine with the same flags plus
+ *                        NB200_FLAG_NO_STREAM.  Positions 0 .. n_prompt-2 run as prefill chunks.  Then at position p (ids[0..p]
+ *                        known): for g = min(ngram_max, p) down to 1, take the largest s <= p-g with ids[s..s+g) ==
+ *                        ids[p-g+1 .. p]; the draft is ids[s+g .. s+g+k) with k = min(draft_max, M-1, n_total-2-p,
+ *                        min(max_seq_len, block_size)-1-p, p+1-(s+g)); the first g giving k >= 1 wins.  With a draft, one
+ *                        nb200_verify_greedy of 1+k positions advances by a+1; without one, one multi-kernel token step (the
+ *                        CUDA graph where the engine has one: launches as one token of that path) advances by 1.
+ *                        stats (optional): [0] verify passes, [1] steps without a draft, [2] drafted ids, [3] accepted ids.
+ *                        prefill_ms / device_ms (optional): CUDA-event time of the prompt and of the decode segment (which
+ *                        includes the host's drafting between passes).  Refuses what nb200_verify_greedy refuses, and
+ *                        ngram_max == 0 or draft_max == 0.
+ * Not covered: sampled speculation (it cannot equal nb200_next_sampled's single coin), verification inside batches, LoRA, tensor
+ * parallelism, non-causal attention, the shim (llm_session_step is one token per call). */
+int nb200_verify_greedy(nb200_engine *e, uint32_t *ids, uint32_t pos, uint32_t n, float repetition_penalty,
+                        uint32_t *n_accepted, float *device_ms);
+int nb200_decode_lookup(nb200_engine *e, uint32_t *ids, uint32_t n_prompt, uint32_t n_total, float repetition_penalty,
+                        uint32_t ngram_max, uint32_t draft_max, uint32_t stats[4], float *prefill_ms, float *device_ms);
 
 /* Batched multi-session decode (no reference counterpart).  A batch is attached to an engine and shares its weights; it holds
  * n_slots sessions ("slots"), each with its own K / V cache (laid out like the engine's and zeroed at creation, n_kv_head *

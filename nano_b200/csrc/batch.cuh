@@ -174,4 +174,18 @@ NB_K __global__ void __launch_bounds__(1024) k_batch_argmax(const BatchArgmaxArg
     }
 }
 
+// Seen rows of a verify pass (nb200_verify_greedy), one CTA per row: row j is the engine's seen set (ids[0..pos)) plus the
+// chunk's ids[0..j) (positions pos .. pos+j-1), so entry j of the pass's classifier penalises exactly what nb200_next_greedy at
+// pos+j would.  The copy, then the marks.
+struct VerifySeenArgs { uint8_t *rows; const uint8_t *seen; const uint32_t *ids; uint32_t V; };
+NB_K __global__ void __launch_bounds__(1024) k_verify_seen(const VerifySeenArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const uint32_t j = blockIdx.x;
+    uint8_t *row = a.rows + (size_t)j * a.V;
+    for (uint32_t i = threadIdx.x; i < a.V; i += 1024) row[i] = a.seen[i];
+    __syncthreads();
+    if (threadIdx.x < j) row[a.ids[threadIdx.x]] = 1;
+}
+
 }  // namespace nb

@@ -149,6 +149,14 @@ struct nb200_engine {
         LayerBufs buf;
         uint32_t *ids = nullptr;
     } pf;
+    // speculative verification (nb200_verify_greedy), allocated on the first call: M logits rows and M seen rows of the pass, its
+    // M greedy ids (pinned host copy), and the K / V rows a pass may overwrite past the accepted ones, [L][KV][M-1][hd] each
+    struct Verify {
+        float *logits = nullptr;
+        uint8_t *seen = nullptr;
+        uint32_t *next = nullptr, *next_host = nullptr;
+        float *ksave = nullptr, *vsave = nullptr;
+    } ver;
 };
 
 namespace {
@@ -851,6 +859,7 @@ void nb200_engine_destroy(nb200_engine *e) {
     for (void *p : e->allocs) cudaFree(p);
     if (e->st_host) cudaFreeHost(e->st_host);
     if (e->samp_host) cudaFreeHost(e->samp_host);
+    if (e->ver.next_host) cudaFreeHost(e->ver.next_host);
     if (e->tok_host) cudaFreeHost(e->tok_host);
     if (e->stream) cudaStreamDestroy(e->stream);
     delete e;
@@ -1825,6 +1834,194 @@ int nb200_batch_read_kv(nb200_batch *b, uint32_t slot, int field, uint32_t layer
     const float *base = (field == NB200_F_KROW ? b->kc : b->vc) + slot * b->slot_elems + (size_t)layer * d.KV * d.max_seq * d.hd;
     for (uint32_t h = 0; h < d.KV; h++)
         CK(cudaMemcpy(dst + (size_t)h * d.hd, base + ((size_t)h * d.max_seq + pos) * d.hd, (size_t)d.hd * 4, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+}  // extern "C"
+
+// ---------------- speculative greedy decoding ----------------
+// A verify pass is a prefill chunk of the consumed id and the drafted ids at pos .. pos+n-1 on the engine's own cache, followed
+// by the batch's classifier and argmax over n entries (slot j = position pos+j, each with its own logits and seen row): the
+// greedy id at every position in one pass over the weights, each bit-identical to nb200_next_greedy there on the multi-kernel path.
+namespace {
+
+// The verify workspace (and prefill's buffers) are allocated on the first call; a failed allocation leaves the engine as it was.
+int verify_setup(nb200_engine *e) {
+    if (e->ver.logits) return 0;
+    int r;
+    if ((r = prefill_setup(e))) return r;
+    const Dims &d = e->d;
+    const uint32_t M = e->pf.M;
+    const size_t save = (size_t)d.L * d.KV * (M - 1) * d.hd * 4;
+    nb200_engine::Verify v;
+    DM(v.logits, (size_t)M * d.V * 4); DM(v.seen, (size_t)M * d.V); DM(v.next, (size_t)M * 4);
+    DM(v.ksave, save); DM(v.vsave, save);
+    CK(cudaHostAlloc(&v.next_host, (size_t)M * 4, cudaHostAllocDefault));
+    e->ver = v;
+    return 0;
+}
+
+// nb200_verify_greedy after its checks
+int verify_pass(nb200_engine *e, uint32_t *ids, uint32_t pos, uint32_t n, float penalty, uint32_t *n_accepted, float *device_ms) {
+    const Dims &d = e->d;
+    const uint32_t M = e->pf.M;
+    const size_t cache_pitch = (size_t)d.max_seq * d.hd * 4, save_pitch = (size_t)(M - 1) * d.hd * 4;
+    auto &v = e->ver;
+    int r;
+    struct Events { cudaEvent_t ev[2] = {nullptr, nullptr}; ~Events() { for (auto x : ev) if (x) cudaEventDestroy(x); } } evs;
+    if (device_ms) for (auto &x : evs.ev) CK(cudaEventCreate(&x));
+    if (penalty != 1.0f) { if ((r = sync_seen(e, ids, pos))) return r; }
+    CK(cudaMemcpyAsync(e->pf.ids, ids + pos, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+    if (device_ms) CK(cudaEventRecord(evs.ev[0], e->stream));
+    if (n > 1) {        // rows pos+1 .. pos+n-1 as they are, for those the pass writes past the accepted ones
+        CK(cudaMemcpy2DAsync(v.ksave, save_pitch, e->kc + (size_t)(pos + 1) * d.hd, cache_pitch, (size_t)(n - 1) * d.hd * 4,
+                             (size_t)d.L * d.KV, cudaMemcpyDeviceToDevice, e->stream));
+        CK(cudaMemcpy2DAsync(v.vsave, save_pitch, e->vc + (size_t)(pos + 1) * d.hd, cache_pitch, (size_t)(n - 1) * d.hd * 4,
+                             (size_t)d.L * d.KV, cudaMemcpyDeviceToDevice, e->stream));
+    }
+    BatchPass bp{};
+    for (uint32_t j = 0; j < n; j++) { bp.slot[j] = j; bp.pos[j] = pos + j; bp.pen[j] = penalty; }
+    if (penalty != 1.0f) {      // x / 1.0f == x: the classifier skips the lookup, as nb200_next_greedy
+        VerifySeenArgs sa{v.seen, e->seen, e->pf.ids, d.V};
+        if ((r = launch<VerifySeenArgs>(e, k_verify_seen, dim3(n), dim3(1024), 0, sa))) return r;
+    }
+    e->pf.attn_kind = pick_attn(e).kind;
+    if ((r = run_prefill_chunk(e, e->kc, e->vc, e->pf.buf, pos, n, e->pf.ids))) return r;
+    BatchMvArgs a{};
+    a.mv.m = n;
+    a.mv.src = e->pf.buf.x; a.mv.src_stride = d.E; a.mv.gain = e->norm_final;
+    a.bp = bp; a.logits = v.logits; a.seen = v.seen;
+    if ((r = run_batch_matvec(e, EPI_CLS, e->cls, a))) return r;
+    BatchArgmaxArgs am{v.logits, bp, v.next, d.V};
+    if ((r = launch<BatchArgmaxArgs>(e, k_batch_argmax, dim3(n), dim3(1024), 0, am))) return r;
+    if (device_ms) CK(cudaEventRecord(evs.ev[1], e->stream));
+    CK(cudaMemcpyAsync(v.next_host, v.next, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    uint32_t acc = 0;
+    while (acc + 1 < n && v.next_host[acc] == ids[pos + acc + 1]) acc++;
+    ids[pos + acc + 1] = v.next_host[acc];
+    // the state nb200_next_greedy at pos .. pos+acc leaves: logits row acc, and rows pos+acc+1 .. pos+n-1 as they were
+    CK(cudaMemcpyAsync(e->logits, v.logits + (size_t)acc * d.V, (size_t)d.V * 4, cudaMemcpyDeviceToDevice, e->stream));
+    if (acc + 1 < n) {
+        const size_t width = (size_t)(n - 1 - acc) * d.hd * 4;
+        CK(cudaMemcpy2DAsync(e->kc + (size_t)(pos + acc + 1) * d.hd, cache_pitch, v.ksave + (size_t)acc * d.hd, save_pitch, width,
+                             (size_t)d.L * d.KV, cudaMemcpyDeviceToDevice, e->stream));
+        CK(cudaMemcpy2DAsync(e->vc + (size_t)(pos + acc + 1) * d.hd, cache_pitch, v.vsave + (size_t)acc * d.hd, save_pitch, width,
+                             (size_t)d.L * d.KV, cudaMemcpyDeviceToDevice, e->stream));
+    }
+    *n_accepted = acc;
+    if (device_ms) CK(cudaEventElapsedTime(device_ms, evs.ev[0], evs.ev[1]));
+    return 0;
+}
+
+int verify_usable(nb200_engine *e) {
+    if (e->tp_size > 1) return fail(NB200_EINVAL, "speculative verification is not available on tensor-parallel engines");
+    if (e->lora.active) return fail(NB200_EINVAL, "speculative verification does not run LoRA plug-ins: disable the plug-in (nb200_lora_enable)");
+    return 0;
+}
+
+// One greedy step at p on the multi-kernel path (nb200_next_greedy's step on a NB200_FLAG_NO_STREAM engine): the captured graph
+// where the engine has one, direct launches otherwise.
+int token_step_multikernel(nb200_engine *e, const uint32_t *ids, uint32_t p, float penalty, uint32_t *next) {
+    int r;
+    if ((r = push_state(e, p, 1, 0, 0, penalty, ids[p], 1))) return r;
+    if (penalty != 1.0f) { if ((r = sync_seen(e, ids, p))) return r; }
+    if (e->graph) {
+        CK(cudaGraphLaunch(e->graph, e->stream));
+        e->launches += e->launches_per_token;
+    } else if ((r = run_token(e))) return r;
+    CK(cudaMemcpyAsync(e->tok_host, &e->st->next_token, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    *next = *e->tok_host;
+    return 0;
+}
+
+// Prompt-lookup draft at p (ids[0..p] known): for g = min(ngram_max, p) down to 1, the largest s <= p-g with
+// ids[s..s+g) == ids[p-g+1..p]; the draft is the k = min(cap, p+1-(s+g)) ids from s+g, and the first g with k >= 1 wins.
+// Returns k (0: no draft) and the draft's start in src.
+uint32_t lookup_draft(const uint32_t *ids, uint32_t p, uint32_t ngram_max, uint32_t cap, uint32_t &src) {
+    for (uint32_t g = ngram_max < p ? ngram_max : p; g >= 1; g--) {
+        for (uint32_t s = p - g + 1; s-- > 0;) {
+            if (memcmp(ids + s, ids + p - g + 1, (size_t)g * 4) != 0) continue;
+            const uint32_t room = p + 1 - (s + g), k = cap < room ? cap : room;
+            if (k >= 1) { src = s + g; return k; }
+            break;
+        }
+    }
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int nb200_verify_greedy(nb200_engine *e, uint32_t *ids, uint32_t pos, uint32_t n, float repetition_penalty,
+                        uint32_t *n_accepted, float *device_ms) {
+    if (!e || !ids || !n_accepted) return fail(NB200_EINVAL, "null argument");
+    int r;
+    if ((r = verify_usable(e))) return r;
+    CK(cudaSetDevice(e->device));
+    uint32_t M = e->pf.M;
+    if (!M && (r = chunk_positions(e, M))) return r;
+    if (n == 0 || n > M) return fail(NB200_EINVAL, "verify of %u positions: a pass verifies 1 .. M = %u positions", n, M);
+    const uint32_t lim = pos_limit(e->d);
+    if (pos >= lim || n > lim - pos)
+        return fail(NB200_EINVAL, "verify of %u positions from %u: past min(max_seq_len, block_size) = %u", n, pos, lim);
+    for (uint32_t p = (repetition_penalty != 1.0f) ? 0 : pos; p < pos + n; p++)      // the penalty reads ids[0..pos)
+        if (ids[p] >= e->d.V) return fail(NB200_EINVAL, "id %u at position %u out of range", ids[p], p);
+    if ((r = verify_setup(e))) return r;
+    return verify_pass(e, ids, pos, n, repetition_penalty, n_accepted, device_ms);
+}
+
+int nb200_decode_lookup(nb200_engine *e, uint32_t *ids, uint32_t n_prompt, uint32_t n_total, float repetition_penalty,
+                        uint32_t ngram_max, uint32_t draft_max, uint32_t stats[4], float *prefill_ms, float *device_ms) {
+    if (!e || !ids) return fail(NB200_EINVAL, "null argument");
+    const uint32_t lim = pos_limit(e->d);
+    if (n_prompt < 1 || n_total < n_prompt || n_total > lim + 1) return fail(NB200_EINVAL, "bad n_prompt/n_total");
+    if (ngram_max == 0 || draft_max == 0) return fail(NB200_EINVAL, "ngram_max and draft_max must be at least 1");
+    int r;
+    if ((r = verify_usable(e))) return r;
+    for (uint32_t i = 0; i < n_prompt; i++) if (ids[i] >= e->d.V) return fail(NB200_EINVAL, "id out of range");
+    CK(cudaSetDevice(e->device));
+    if ((r = verify_setup(e))) return r;
+    struct Events { cudaEvent_t ev[3] = {nullptr, nullptr, nullptr}; ~Events() { for (auto v : ev) if (v) cudaEventDestroy(v); } } evs;
+    for (auto &v : evs.ev) CK(cudaEventCreate(&v));
+    const uint32_t M = e->pf.M, np = n_prompt - 1;
+    if (np) CK(cudaMemcpyAsync(e->pf.ids, ids, (size_t)np * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaEventRecord(evs.ev[0], e->stream));
+    if (np) e->pf.attn_kind = pick_attn(e).kind;
+    for (uint32_t c = 0; c < np; c += M) {
+        const uint32_t m = (np - c < M) ? np - c : M;
+        if ((r = run_prefill_chunk(e, e->kc, e->vc, e->pf.buf, c, m, e->pf.ids + c))) return r;
+    }
+    CK(cudaEventRecord(evs.ev[1], e->stream));
+    uint32_t st[4] = {0, 0, 0, 0};
+    for (uint32_t p = np; p + 1 < n_total;) {
+        uint32_t cap = draft_max, src = 0;
+        if (cap > M - 1) cap = M - 1;
+        if (cap > n_total - 2 - p) cap = n_total - 2 - p;
+        if (cap > lim - 1 - p) cap = lim - 1 - p;
+        const uint32_t k = lookup_draft(ids, p, ngram_max, cap, src);
+        if (k) {
+            memmove(ids + p + 1, ids + src, (size_t)k * 4);
+            uint32_t a = 0;
+            if ((r = verify_pass(e, ids, p, 1 + k, repetition_penalty, &a, nullptr))) return r;
+            st[0]++; st[2] += k; st[3] += a;
+            p += a + 1;
+        } else {
+            if ((r = token_step_multikernel(e, ids, p, repetition_penalty, &ids[p + 1]))) return r;
+            st[1]++;
+            p++;
+        }
+    }
+    CK(cudaEventRecord(evs.ev[2], e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    float a = 0, b = 0;
+    CK(cudaEventElapsedTime(&a, evs.ev[0], evs.ev[1]));
+    CK(cudaEventElapsedTime(&b, evs.ev[1], evs.ev[2]));
+    if (prefill_ms) *prefill_ms = a;
+    if (device_ms) *device_ms = b;
+    if (stats) memcpy(stats, st, sizeof st);
     return 0;
 }
 

@@ -25,7 +25,7 @@ MATVEC_EPILOGUES = ("store", "qkv", "resid", "swiglu", "cls")      # kernels.cuh
 EXPORTS = [
     "nb200_last_error", "nb200_device_count", "nb200_engine_create", "nb200_engine_destroy", "nb200_get_config",
     "nb200_forward", "nb200_read_logits", "nb200_next_greedy", "nb200_next_sampled", "nb200_decode_greedy", "nb200_prefill",
-    "nb200_read_buffer",
+    "nb200_verify_greedy", "nb200_decode_lookup", "nb200_read_buffer",
     "nb200_write_x", "nb200_run_layer", "nb200_profile_tokens", "nb200_trace_token", "nb200_read_attn_trace", "nb200_kernel_launches", "nb200_launches_per_token", "nb200_weight_bytes",
     "nb200_op_rmsnorm", "nb200_op_q80_quantize", "nb200_op_q80_matvec", "nb200_op_f32_matvec",
     "nb200_op_q4k_quantize", "nb200_op_q4k_matvec",
@@ -73,6 +73,8 @@ def lib():
         L.nb200_next_sampled.argtypes = [C.c_void_p, u32p, C.c_uint32, C.c_float, C.c_float, C.c_float, C.c_float, u32p, u32p]
         L.nb200_decode_greedy.argtypes = [C.c_void_p, u32p, C.c_uint32, C.c_uint32, C.c_float, f32p, f32p]
         L.nb200_prefill.argtypes = [C.c_void_p, u32p, C.c_uint32, C.c_uint32, f32p]
+        L.nb200_verify_greedy.argtypes = [C.c_void_p, u32p, C.c_uint32, C.c_uint32, C.c_float, u32p, f32p]
+        L.nb200_decode_lookup.argtypes = [C.c_void_p, u32p, C.c_uint32, C.c_uint32, C.c_float, C.c_uint32, C.c_uint32, u32p, f32p, f32p]
         L.nb200_read_buffer.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32]
         L.nb200_write_x.argtypes = [C.c_void_p, f32p, C.c_uint32]
         L.nb200_run_layer.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]
@@ -269,6 +271,28 @@ class Engine:
         ms = C.c_float(0)
         _check(lib().nb200_prefill(self.h, _p(ids, u32p), int(pos0), int(n), C.byref(ms)))
         return float(ms.value)
+
+    def verify_greedy(self, ids: np.ndarray, pos: int, n: int, penalty: float = 1.0) -> int:
+        """Speculative verification of the n-1 drafted ids ids[pos+1:pos+n] in one pass: returns the number a accepted and writes
+        the greedy id at pos+a into ids[pos+a+1] in place (ids: uint32, at least pos+n+1 entries).  The device time of the pass
+        is left in self.verify_ms."""
+        assert ids.dtype == np.uint32 and ids.flags.c_contiguous and ids.size >= pos + n + 1
+        acc, ms = C.c_uint32(0), C.c_float(0)
+        _check(lib().nb200_verify_greedy(self.h, _p(ids, u32p), int(pos), int(n), penalty, C.byref(acc), C.byref(ms)))
+        self.verify_ms = float(ms.value)
+        return int(acc.value)
+
+    def decode_lookup(self, ids: np.ndarray, n_prompt: int, n_total: int, penalty: float = 1.0, ngram_max: int = 3,
+                      draft_max: Optional[int] = None):
+        """decode_greedy with drafts looked up in the context and verified (nb200_decode_lookup): fills ids[n_prompt:n_total] in
+        place with decode_greedy's ids.  draft_max None: the chunk size - 1.  Returns ([verify passes, steps without a draft,
+        drafted ids, accepted ids], prefill_ms, decode_ms)."""
+        assert ids.dtype == np.uint32 and ids.flags.c_contiguous and ids.size >= n_total
+        stats = np.zeros(4, np.uint32)
+        a, b = C.c_float(0), C.c_float(0)
+        _check(lib().nb200_decode_lookup(self.h, _p(ids, u32p), int(n_prompt), int(n_total), penalty, int(ngram_max),
+                                         0xffffffff if draft_max is None else int(draft_max), _p(stats, u32p), C.byref(a), C.byref(b)))
+        return stats.tolist(), float(a.value), float(b.value)
 
     def read(self, field: int, count: int, layer: int = 0, pos: int = 0, dtype=np.float32) -> np.ndarray:
         out = np.zeros(count, dtype=dtype)
