@@ -113,6 +113,7 @@ struct nb200_engine {
     // grid-wide persistent streaming kernel (stream.cuh): the default path in fast mode on one GPU
     float calib_ms[2] = {0.0f, 0.0f};      // ms per token of {streaming, multi-kernel} measured by calibrate_paths (0 = not calibrated)
     bool use_stream = false; const void *st_kern = nullptr; StreamArgs sa{}; uint32_t st_smem = 0, st_grid = 0;
+    bool st_width_fixed = false;                                 // NB200_STREAM_WIDTH chose st_grid (no width calibration)
     uint32_t *st_err_host = nullptr, *st_err_dev = nullptr;      // mapped pinned word: the code a device-side spin recorded before trapping
     uint32_t st_epoch = 0;                                       // exchange epochs handed out so far (stream.cuh)
     void *samp_ws = nullptr; size_t samp_cub = 0; uint32_t *samp_host = nullptr;       // device-side sampler workspace (sample.cu), pinned result
@@ -684,6 +685,94 @@ int put_rows(nb200_engine *e, Mat &m, const uint8_t *w, const uint8_t *aux, uint
 // ---------------- streaming path: per-CTA tile-ordered weight stream + schedule (stream.cuh) ----------------
 uint32_t env_u32(const char *name, uint32_t dflt) { const char *s = getenv(name); return (s && *s) ? (uint32_t)strtoul(s, nullptr, 10) : dflt; }
 
+// Grid width of the streaming kernel.  A grid of W <= num_sms CTAs computes the bits a grid of num_sms computes:
+//  - Rows: CTA c owns units [c * units / W, (c + 1) * units / W) of every kind, and no row's value depends on the CTA, the tile
+//    or the team that computes it.  The shared-tile Q80 dot (st_row_q80_lpg) adds exact integer group sums in group order for
+//    any team geometry (StGeo), the owned-tile one (st_rows_q80_warp) keeps one partial per lane over k = 16 lane + 512 i and
+//    one butterfly for any row block, and F32 / Q4K rows run st_row_f32 / st_row_q4k on both kinds of tile.  The one choice
+//    that changes a row's fp32 order is Q80's shared vs owned form, so st_layout makes it from the rows per CTA at num_sms.
+//  - Attention: nsplit_max and chunk_target do not depend on W, and CTA i runs (kv head, split) item i, so W must be at least
+//    KV * nsplit at the longest range (nsplit <= the split count st_attn_plan starts from, monotonic in the range).
+//  - Every CTA merges the per-CTA classifier partials by (value, lowest index): the same id for any W.
+//  - A CTA keeps at most kStOwnMax residual rows.
+uint32_t st_width_min(const nb200_engine *e) {
+    const Dims &d = e->d;
+    const StreamArgs &g = e->sa;
+    uint32_t ns = (d.max_seq + g.chunk_target - 1) / g.chunk_target;      // non-causal steps attend over max_seq rows
+    if (ns < 1) ns = 1;
+    if (ns > g.nsplit_max) ns = g.nsplit_max;
+    uint32_t w = d.KV * ns;
+    const uint32_t own = (d.E + kStOwnMax - 1) / kStOwnMax;
+    return w > own ? w : own;
+}
+
+// Per-CTA row slices, tiles and the tile-ordered stream copy of the weights for a grid of W CTAs (replaces an earlier copy).
+int st_layout(nb200_engine *e, uint32_t W) {
+    const Dims &d = e->d;
+    StreamArgs &g = e->sa;
+    if (g.stream) {
+        for (auto it = e->allocs.begin(); it != e->allocs.end(); ++it) if (*it == (const void *)g.stream) { e->allocs.erase(it); break; }
+        CK(cudaFree((void *)g.stream));
+        g.stream = nullptr;
+    }
+    const uint32_t NS = (uint32_t)e->num_sms;
+    uint64_t off = 0;
+    uint32_t ntl[5];
+    for (int i = 0; i < 5; i++) {
+        StKind &sk = g.kind[i];
+        const uint32_t rowb = sk.row_stride + sk.aux_stride;
+        const uint32_t max_rows = ((sk.units + W - 1) / W) * sk.unit_rows;
+        const uint32_t rows_ns = ((sk.units + NS - 1) / NS) * sk.unit_rows;
+        uint32_t T = (g.stage_bytes - 16u) / rowb;
+        T -= T % sk.unit_rows;
+        if (T > max_rows) T = max_rows;
+        // many rows per CTA: throughput mode, every tile is consumed by one warp -- small tiles so that all 15 warps have one.
+        // 64 rows: measured on H100 against 16 / 32 (Nano-168M Q80 1519 vs 1473 / 1443 tok/s, Qwen3-0.6B Q4K 892 vs 879 / 886).
+        // Decided at width num_sms for every W: the two forms sum a Q80 row in different fp32 orders.
+        sk.owned = (rows_ns >= env_u32("NB200_OWNED_ROWS", 64) || (uint64_t)rows_ns * rowb >= (uint64_t)env_u32("NB200_OWNED_KB", 32) * 1024u) ? 1u : 0u;
+        if (sk.owned) {
+            uint32_t t2 = (max_rows + kConsWarps - 1) / kConsWarps;
+            t2 = ((t2 + sk.unit_rows - 1) / sk.unit_rows) * sk.unit_rows;
+            if (t2 < 2u) t2 = 2u;
+            if (t2 < T) T = t2;
+        }
+        sk.tile_rows = T;
+        sk.tile_stride = (T * rowb + 15u) & ~15u;
+        ntl[i] = (max_rows + T - 1) / T;
+        if (i == SK_CLS) off = 0;
+        sk.off = off;
+        off += (uint64_t)ntl[i] * sk.tile_stride;
+        off = (off + 127u) & ~(uint64_t)127u;
+        if (i == SK_W2) g.layer_stride = off;
+    }
+    g.cls_off = (uint64_t)d.L * g.layer_stride;
+    g.kind[SK_CLS].off = 0;
+    g.cta_stride = (g.cls_off + (uint64_t)ntl[SK_CLS] * g.kind[SK_CLS].tile_stride + 127u) & ~(uint64_t)127u;
+
+    uint8_t *stream = nullptr;
+    const uint64_t total = g.cta_stride * W + 256;
+    DM(stream, total);
+    g.stream = stream;
+    CK(cudaMemset(stream, 0, total));
+    auto build = [&](int ki, const Mat &m, uint64_t base_off) -> int {
+        const StKind &sk = g.kind[ki];
+        const uint32_t aux_b = (d.quant == 0x80u) ? (sk.n / d.gs) * 4u : sk.aux_stride;
+        uint32_t gx = ((sk.units + W - 1) / W) * sk.unit_rows; if (gx > 1024) gx = 1024; if (gx < 1) gx = 1;
+        CK(stream_build_launch((const uint8_t *)m.w, (const uint8_t *)m.aux, sk.row_stride - 16u, aux_b, sk, stream, g.cta_stride, base_off, gx, W));
+        return 0;
+    };
+    int r;
+    for (uint32_t l = 0; l < d.L; l++) {
+        const uint64_t lb = (uint64_t)l * g.layer_stride;
+        if ((r = build(SK_QKV, e->qkv[l], lb)) || (r = build(SK_O, e->wo[l], lb)) || (r = build(SK_W13, e->w13[l], lb)) || (r = build(SK_W2, e->w2[l], lb))) return r;
+    }
+    if ((r = build(SK_CLS, e->cls, g.cls_off))) return r;
+    CK(cudaDeviceSynchronize());
+    e->stream_bytes = total;
+    e->st_grid = W;
+    return 0;
+}
+
 // returns 0 and sets e->use_stream when the model fits the streaming kernel; 0 without setting it otherwise
 int setup_stream(nb200_engine *e) {
     const Dims &d = e->d;
@@ -698,21 +787,20 @@ int setup_stream(nb200_engine *e) {
     if (!coop) return 0;
     const uint32_t NC = (uint32_t)e->num_sms;
     if (d.KV > NC || (d.E + NC - 1) / NC > (uint32_t)kStOwnMax) return 0;
-    const uint32_t L = d.L;
 
     StreamArgs &g = e->sa;
     memset(&g, 0, sizeof g);
     struct KM { uint32_t rows, n, unit; } km[5] = {
         {d.q_dim + 2 * d.kv_dim, d.E, 1}, {d.E, d.q_dim, 1}, {2 * d.F, d.E, 2}, {d.E, d.F, 1}, {d.V, d.E, 1}};
-    uint32_t main_b[5], aux_b[5], unit_b_max = 0;
+    uint32_t unit_b_max = 0;
     for (int i = 0; i < 5; i++) {
         const uint32_t n = km[i].n;
-        main_b[i] = (d.quant == 0x00u) ? n * 4u : (d.quant == 0x80u) ? n : n / 2u;
-        aux_b[i] = (d.quant == 0x00u) ? 0u : (d.quant == 0x80u) ? (n / d.gs) * 4u : (n / 256u) * 20u;
+        const uint32_t main_b = (d.quant == 0x00u) ? n * 4u : (d.quant == 0x80u) ? n : n / 2u;
+        const uint32_t aux_b = (d.quant == 0x00u) ? 0u : (d.quant == 0x80u) ? (n / d.gs) * 4u : (n / 256u) * 20u;
         StKind &sk = g.kind[i];
         sk.units = km[i].rows / km[i].unit; sk.unit_rows = km[i].unit; sk.n = n;
-        sk.row_stride = main_b[i] + 16u;
-        sk.aux_stride = (d.quant == 0x80u) ? ((n / d.gs) | 1u) * 4u : aux_b[i];
+        sk.row_stride = main_b + 16u;
+        sk.aux_stride = (d.quant == 0x80u) ? ((n / d.gs) | 1u) * 4u : aux_b;
         const uint32_t ub = km[i].unit * (sk.row_stride + sk.aux_stride);
         if (ub > unit_b_max) unit_b_max = ub;
     }
@@ -744,37 +832,11 @@ int setup_stream(nb200_engine *e) {
         if (stage_bytes < min_stage + 1024u) return 0;
     }
     g.off_ring = region0;
-    uint64_t off = 0;
-    uint32_t ntl[5];
-    for (int i = 0; i < 5; i++) {
-        StKind &sk = g.kind[i];
-        const uint32_t rowb = sk.row_stride + sk.aux_stride;
-        const uint32_t max_rows = ((sk.units + NC - 1) / NC) * sk.unit_rows;
-        uint32_t T = (stage_bytes - 16u) / rowb;
-        T -= T % sk.unit_rows;
-        if (T > max_rows) T = max_rows;
-        if (T < sk.unit_rows) return 0;
-        // many rows per CTA: throughput mode, every tile is consumed by one warp -- small tiles so that all 15 warps have one.
-        // 64 rows: measured on H100 against 16 / 32 (Nano-168M Q80 1519 vs 1473 / 1443 tok/s, Qwen3-0.6B Q4K 892 vs 879 / 886)
-        sk.owned = (max_rows >= env_u32("NB200_OWNED_ROWS", 64) || (uint64_t)max_rows * rowb >= (uint64_t)env_u32("NB200_OWNED_KB", 32) * 1024u) ? 1u : 0u;
-        if (sk.owned) {
-            uint32_t t2 = (max_rows + kConsWarps - 1) / kConsWarps;
-            t2 = ((t2 + sk.unit_rows - 1) / sk.unit_rows) * sk.unit_rows;
-            if (t2 < 2u) t2 = 2u;
-            if (t2 < T) T = t2;
-        }
-        sk.tile_rows = T;
-        sk.tile_stride = (T * rowb + 15u) & ~15u;
-        ntl[i] = (max_rows + T - 1) / T;
-        if (i == SK_CLS) off = 0;
-        sk.off = off;
-        off += (uint64_t)ntl[i] * sk.tile_stride;
-        off = (off + 127u) & ~(uint64_t)127u;
-        if (i == SK_W2) g.layer_stride = off;
+    for (int i = 0; i < 5; i++) {                       // a stage holds one row unit of every kind (tiles: st_layout)
+        const StKind &sk = g.kind[i];
+        const uint32_t T = (stage_bytes - 16u) / (sk.row_stride + sk.aux_stride);
+        if (T - T % sk.unit_rows < sk.unit_rows) return 0;
     }
-    g.cls_off = (uint64_t)L * g.layer_stride;
-    g.kind[SK_CLS].off = 0;
-    g.cta_stride = (g.cls_off + (uint64_t)ntl[SK_CLS] * g.kind[SK_CLS].tile_stride + 127u) & ~(uint64_t)127u;
 
     const uint32_t smem = region0 + nst * stage_bytes;
     cudaError_t ce = cudaFuncSetAttribute((const void *)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -782,37 +844,18 @@ int setup_stream(nb200_engine *e) {
     if (ce == cudaSuccess) ce = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (const void *)k, kThreads, smem);
     if (ce != cudaSuccess || occ < 1) { cudaGetLastError(); return 0; }
 
-    // device objects: the stream copy of the weights
-    uint8_t *stream = nullptr;
-    const uint64_t total = g.cta_stride * NC + 256;
-    DM(stream, total);
-    CK(cudaMemset(stream, 0, total));
-    auto build = [&](int ki, const Mat &m, uint64_t base_off) -> int {
-        const StKind &sk = g.kind[ki];
-        uint32_t gx = ((sk.units + NC - 1) / NC) * sk.unit_rows; if (gx > 1024) gx = 1024; if (gx < 1) gx = 1;
-        CK(stream_build_launch((const uint8_t *)m.w, (const uint8_t *)m.aux, main_b[ki], aux_b[ki], sk, stream, g.cta_stride, base_off, gx, NC));
-        return 0;
-    };
-    int r;
-    for (uint32_t l = 0; l < L; l++) {
-        const uint64_t lb = (uint64_t)l * g.layer_stride;
-        if ((r = build(SK_QKV, e->qkv[l], lb)) || (r = build(SK_O, e->wo[l], lb)) || (r = build(SK_W13, e->w13[l], lb)) || (r = build(SK_W2, e->w2[l], lb))) return r;
-    }
-    if ((r = build(SK_CLS, e->cls, g.cls_off))) return r;
-    CK(cudaDeviceSynchronize());
-    e->stream_bytes = total;
-
     if (!e->bar) { DM(e->bar, 64); CK(cudaMemset(e->bar, 0, 64)); }
     CK(cudaHostAlloc(&e->st_err_host, 64, cudaHostAllocMapped));
     memset(e->st_err_host, 0, 64);
     CK(cudaHostGetDevicePointer((void **)&e->st_err_dev, e->st_err_host, 0));
 
-    g.stream = stream; g.nstages = nst; g.stage_bytes = stage_bytes; g.kv_tile_rows = kv_rows;
+    g.nstages = nst; g.stage_bytes = stage_bytes; g.kv_tile_rows = kv_rows;
     g.kv_tile_magic = (uint32_t)((0x100000000ull + kv_rows - 1) / kv_rows);
     g.g_attn = e->norm_attn; g.g_ffn = e->norm_ffn; g.g_final = e->norm_final;
     g.qnorm = e->qnorm; g.knorm = e->knorm; g.rope_cos = e->rope_cos; g.rope_sin = e->rope_sin;
     g.emb_w = e->emb.w; g.emb_aux = e->emb.aux;
     g.logits = e->logits; g.kc = e->kc; g.vc = e->vc;
+    int r;
     {   // activation exchange words {value, epoch}, zeroed once: epoch 0 is never handed out
         auto words = [&](unsigned long long *&p, size_t n) -> int { DM(p, n * 8 + 256); CK(cudaMemset(p, 0, n * 8 + 256)); return 0; };
         const uint32_t ns[3] = {d.E, d.q_dim, d.F};
@@ -831,7 +874,18 @@ int setup_stream(nb200_engine *e) {
     g.ablate = env_u32("NB200_ABLATE", 0);
     if (g.chunk_target < 8) g.chunk_target = 8;
     g.d = d;
-    e->st_kern = (const void *)k; e->st_smem = smem; e->st_grid = NC; e->use_stream = true; e->launches_per_token = 1;
+
+    // NB200_STREAM_WIDTH=<W> fixes the grid width (tests, sweeps); otherwise calibrate_width picks it after creation
+    uint32_t W = NC;
+    const char *wenv = getenv("NB200_STREAM_WIDTH");
+    if (wenv && *wenv) {
+        W = (uint32_t)strtoul(wenv, nullptr, 10);
+        const uint32_t wmin = st_width_min(e);
+        if (W < wmin || W > NC) return fail(NB200_EINVAL, "NB200_STREAM_WIDTH=%s: this model's streaming kernel runs on %u..%u CTAs", wenv, wmin, NC);
+        e->st_width_fixed = true;
+    }
+    if ((r = st_layout(e, W))) return r;
+    e->st_kern = (const void *)k; e->st_smem = smem; e->use_stream = true; e->launches_per_token = 1;
     return 0;
 }
 
@@ -867,6 +921,7 @@ void nb200_engine_destroy(nb200_engine *e) {
 
 static int finish_paths(nb200_engine *e);
 static int calibrate_paths(nb200_engine *e);
+static int calibrate_width(nb200_engine *e);
 static int push_state(nb200_engine *e, uint32_t pos, uint32_t causal, uint32_t n_prompt, uint32_t advance, float penalty,
                       uint32_t token, uint32_t use_token);
 
@@ -1138,6 +1193,7 @@ static int create_impl(nb200_engine **out, const uint8_t *img, uint64_t image_by
         if (T == 1 && !st_off) { if ((r = setup_stream(e))) return r; }
         e->path_stream = e->use_stream;
         if (T == 1 && (r = finish_paths(e))) return r;      // tensor-parallel engines capture after the peers are attached
+        if (e->use_stream && !e->st_width_fixed && (r = calibrate_width(e))) return r;
         const bool st_always = d.quant != 0x80u || e->weight_bytes < (256ull << 20);
         if (e->use_stream && !st_forced && !st_always && (r = calibrate_paths(e))) return r;
     }
@@ -1163,37 +1219,28 @@ static int finish_paths(nb200_engine *e) {
     return 0;
 }
 
-// Both fast paths are ready: time `n` decode steps on each from the middle of the usable context (device loop, CUDA events on the
-// engine's stream, one untimed round first) and keep the faster.  The steps write K/V rows at positions pos0.., logits, x and the
-// ids; all of it is cleared again afterwards, because non-causal attention reads every cache row, written or not, and a fresh
-// engine must compute what the reference's calloc'd context does.
-static int calibrate_paths(nb200_engine *e) {
-    const uint32_t n = 8;
-    const uint32_t lim = pos_limit(e->d);
-    if (lim < 4 * n) return 0;
-    const uint32_t pos0 = lim / 2;
+// Decode steps at positions pos0 .. pos0 + n - 1 on the current path, timed with CUDA events on the engine's stream; ms is the
+// second of two identical rounds.  The steps write K/V rows, logits, x and the ids: clear_session undoes that.
+static int time_steps(nb200_engine *e, uint32_t pos0, uint32_t n, float &ms) {
     struct Events { cudaEvent_t ev[2] = {nullptr, nullptr}; ~Events() { for (auto v : ev) if (v) cudaEventDestroy(v); } } evs;
     for (auto &v : evs.ev) CK(cudaEventCreate(&v));
-    float ms[2] = {0.0f, 0.0f};
     int r;
-    for (int path = 0; path < 2; path++) {
-        e->use_stream = (path == 0);
-        if (path == 1) { e->launches_per_token = 0; if ((r = finish_paths(e))) return r; }      // captures the multi-kernel graph
-        for (int rep = 0; rep < 2; rep++) {
-            CK(cudaMemsetAsync(e->ids_dev, 0, (size_t)(pos0 + 1) * 4, e->stream));
-            if ((r = push_state(e, pos0, 1, pos0 + 1, 1, 1.0f, 0, 0))) return r;
-            CK(cudaEventRecord(evs.ev[0], e->stream));
-            if (e->use_stream) { if ((r = launch_stream(e, n))) return r; }
-            else for (uint32_t i = 0; i < n; i++) if ((r = launch_token(e))) return r;
-            CK(cudaEventRecord(evs.ev[1], e->stream));
-            CK(cudaStreamSynchronize(e->stream));
-            CK(cudaEventElapsedTime(&ms[path], evs.ev[0], evs.ev[1]));
-        }
+    for (int rep = 0; rep < 2; rep++) {
+        CK(cudaMemsetAsync(e->ids_dev, 0, (size_t)(pos0 + 1) * 4, e->stream));
+        if ((r = push_state(e, pos0, 1, pos0 + 1, 1, 1.0f, 0, 0))) return r;
+        CK(cudaEventRecord(evs.ev[0], e->stream));
+        if (e->use_stream) { if ((r = launch_stream(e, n))) return r; }
+        else for (uint32_t i = 0; i < n; i++) if ((r = launch_token(e))) return r;
+        CK(cudaEventRecord(evs.ev[1], e->stream));
+        CK(cudaStreamSynchronize(e->stream));
+        CK(cudaEventElapsedTime(&ms, evs.ev[0], evs.ev[1]));
     }
-    e->calib_ms[0] = ms[0] / n; e->calib_ms[1] = ms[1] / n;
-    e->use_stream = ms[0] <= ms[1];
-    e->path_stream = e->use_stream;
-    if (e->use_stream) e->launches_per_token = 1;
+    return 0;
+}
+
+// Back to the state of a fresh engine: non-causal attention reads every cache row, written or not, and a fresh engine must
+// compute what the reference's calloc'd context does.
+static int clear_session(nb200_engine *e) {
     e->launches = 0;
     const Dims &d = e->d;                                                                 // as created
     const size_t kv_floats = (size_t)d.L * d.KV * d.max_seq * d.hd;
@@ -1204,6 +1251,50 @@ static int calibrate_paths(nb200_engine *e) {
     e->seen_valid = false; e->seen_mirror.clear();
     CK(cudaStreamSynchronize(e->stream));
     return 0;
+}
+
+// Both fast paths are ready: time `n` decode steps on each from the middle of the usable context and keep the faster.
+static int calibrate_paths(nb200_engine *e) {
+    const uint32_t n = 8;
+    const uint32_t lim = pos_limit(e->d);
+    if (lim < 4 * n) return 0;
+    float ms[2] = {0.0f, 0.0f};
+    int r;
+    for (int path = 0; path < 2; path++) {
+        e->use_stream = (path == 0);
+        if (path == 1) { e->launches_per_token = 0; if ((r = finish_paths(e))) return r; }      // captures the multi-kernel graph
+        if ((r = time_steps(e, lim / 2, n, ms[path]))) return r;
+    }
+    e->calib_ms[0] = ms[0] / n; e->calib_ms[1] = ms[1] / n;
+    e->use_stream = ms[0] <= ms[1];
+    e->path_stream = e->use_stream;
+    if (e->use_stream) e->launches_per_token = 1;
+    return clear_session(e);
+}
+
+// The streaming kernel is ready at num_sms CTAs: time it as calibrate_paths does at num_sms and at 15/16, 7/8, 3/4, 1/2 and
+// 1/3 of it, as far down as st_width_min allows, and keep the fastest width (the bits are the same at every width,
+// st_width_min).  A narrower grid has fewer CTAs to exchange with and wait for in every phase, and more rows per CTA; where a
+// phase's rows per CTA outgrow one ring tile, the time steps up (DESIGN.md section 5.4: Nano-168M Q80 is fastest from 110 to
+// 128 CTAs of 132).  Each width needs its own stream copy of the weights (st_layout), built in place.
+static int calibrate_width(nb200_engine *e) {
+    const uint32_t n = 8;
+    const uint32_t lim = pos_limit(e->d);
+    const uint32_t NS = (uint32_t)e->num_sms, wmin = st_width_min(e);
+    const uint32_t cand[6] = {NS, (15 * NS) / 16, (7 * NS) / 8, (3 * NS) / 4, NS / 2, NS / 3};
+    if (lim < 4 * n || cand[1] < wmin) return 0;
+    uint32_t best_w = e->st_grid;
+    float best = 0.0f;
+    int r;
+    for (uint32_t W : cand) {
+        if (W < wmin) break;
+        if (W != e->st_grid && (r = st_layout(e, W))) return r;
+        float ms = 0.0f;
+        if ((r = time_steps(e, lim / 2, n, ms))) return r;
+        if (best == 0.0f || ms < best) { best = ms; best_w = W; }
+    }
+    if (best_w != e->st_grid && (r = st_layout(e, best_w))) return r;
+    return clear_session(e);
 }
 
 int nb200_engine_create(nb200_engine **out, const uint8_t *img, uint64_t image_bytes, uint32_t max_seq_len, int device,
@@ -1341,7 +1432,7 @@ int nb200_get_config(const nb200_engine *e, nb200_config *c) {
     c->block_size = d.block_size; c->vocab_size = d.V; c->n_layer = d.L; c->n_embd = d.E;
     c->n_head = e->g_H; c->n_kv_head = e->g_KV; c->n_hidden = d.F; c->tied = e->tied ? 1u : 0u; c->head_dim = d.hd;
     c->q_dim = e->g_q_dim; c->kv_dim = e->g_kv_dim; c->max_seq_len = d.max_seq; c->tp_rank = e->tp_rank; c->tp_size = e->tp_size;
-    c->reserved[0] = e->use_stream ? 4u : (e->graph ? 1u : 0u);      // execution path: 4 streaming kernel, 1 graph, 0 direct launches
+    c->reserved[0] = e->use_stream ? 4u | e->st_grid << 8 : (e->graph ? 1u : 0u);    // execution path: 4 | CTAs << 8 streaming kernel, 1 graph, 0 direct launches
     c->reserved[1] = (uint32_t)(e->calib_ms[0] * 1000.0f + 0.5f);     // calibrate_paths: microseconds per token of the streaming kernel ...
     c->reserved[2] = (uint32_t)(e->calib_ms[1] * 1000.0f + 0.5f);     // ... and of the multi-kernel graph (0 = the choice was not measured)
     c->reserved[3] = e->mv_mask;

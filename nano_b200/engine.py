@@ -159,9 +159,12 @@ class Engine:
             setattr(self, n, int(getattr(cfg, n)))
         self.vocab = self.vocab_size
         self.path = {4: "streaming kernel (persistent grid, per-CTA TMA ring over weights and KV, L2 grid barriers)",
-                     1: "multi-kernel CUDA graph with PDL", 0: "multi-kernel direct launches"}[int(cfg.reserved[0])]
+                     1: "multi-kernel CUDA graph with PDL", 0: "multi-kernel direct launches"}[int(cfg.reserved[0]) & 0xff]
+        # streaming kernel: CTAs of its grid (NB200_STREAM_WIDTH, or the fastest width timed at creation); None on the other paths
+        self.stream_width = (int(cfg.reserved[0]) >> 8) or None
         # creation-time calibration of the two fast paths (large one-GPU Q80 engines): us per token of each, None when not measured
-        self.calibration = ({"streaming_us_per_token": int(cfg.reserved[1]), "multikernel_us_per_token": int(cfg.reserved[2])}
+        self.calibration = ({"streaming_us_per_token": int(cfg.reserved[1]), "multikernel_us_per_token": int(cfg.reserved[2]),
+                             "stream_width": self.stream_width}
                             if int(cfg.reserved[1]) and int(cfg.reserved[2]) else None)
 
     def kernels(self) -> dict:
