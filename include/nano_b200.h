@@ -201,8 +201,8 @@ int nb200_prefill(nb200_engine *e, const uint32_t *ids, uint32_t pos0, uint32_t 
  *                        prefill_ms / device_ms (optional): CUDA-event time of the prompt and of the decode segment (which
  *                        includes the host's drafting between passes).  Refuses what nb200_verify_greedy refuses, and
  *                        ngram_max == 0 or draft_max == 0.
- * Not covered: sampled speculation (it cannot equal nb200_next_sampled's single coin), verification inside batches, LoRA, tensor
- * parallelism, non-causal attention, the shim (llm_session_step is one token per call). */
+ * Not covered: sampled speculation (it cannot equal nb200_next_sampled's single coin), LoRA, tensor parallelism, non-causal
+ * attention, the shim (llm_session_step is one token per call).  Batched verification: nb200_batch_verify_greedy below. */
 int nb200_verify_greedy(nb200_engine *e, uint32_t *ids, uint32_t pos, uint32_t n, float repetition_penalty,
                         uint32_t *n_accepted, float *device_ms);
 int nb200_decode_lookup(nb200_engine *e, uint32_t *ids, uint32_t n_prompt, uint32_t n_total, float repetition_penalty,
@@ -229,6 +229,29 @@ int nb200_decode_lookup(nb200_engine *e, uint32_t *ids, uint32_t n_prompt, uint3
  *                            allocation fails the call before anything is written) and freed by nb200_batch_destroy; the
  *                            engine's own sampler workspace is never used.  A sampled entry's result depends neither on the
  *                            other entries of the call nor on which of them sample.
+ *   nb200_batch_verify_greedy entry i does in slot slots[i] exactly what nb200_verify_greedy(e, ids[i], pos[i], n_pos[i],
+ *                            repetition_penalty[i], &n_accepted[i]) does on an engine created with the same flags plus
+ *                            NB200_FLAG_NO_STREAM running that session alone: ids[i][pos[i]] is consumed, ids[i][pos[i]+1 ..
+ *                            pos[i]+n_pos[i]) are the drafts, n_accepted[i] = a is the largest count whose greedy ids g_j (j < a)
+ *                            all match their drafts, and ids[i][pos[i]+a+1] receives g_a (ids[i] needs pos[i]+n_pos[i]+1 entries).
+ *                            Afterwards the slot is where nb200_batch_next_greedy at pos .. pos+a leaves it: K/V rows pos .. pos+a
+ *                            written, rows from pos+a+1 on as they were before the call, the slot's logits the penalised row at
+ *                            pos+a, its seen set at ids[0..pos).  An entry with n_pos[i] == 1 is exactly nb200_batch_next_greedy's
+ *                            entry.  Packing: the entries run in call order in passes of at most M rows (info[0]); an entry is
+ *                            never split across passes, and a new pass starts when the next entry's n_pos does not fit in the
+ *                            rows left.  A row's value depends neither on the packing nor on the other entries, so the packing
+ *                            changes only the speed.  Acceptance and the restore of the rows past the accepted ones run on the
+ *                            device: one host synchronise per call, at the end.  Launches per pass: 1 + 6 * n_layer (the chunk,
+ *                            with a K-row pass per layer), + 3 (classifier, argmax, accept), + 1 when an entry of the pass drafts
+ *                            (n_pos > 1: the save of the rows it overwrites), + 1 when an entry of the pass has repetition_penalty
+ *                            != 1 (its seen rows); plus, per call, nb200_batch_next_greedy's seen-set update of each penalised slot
+ *                            whose ids[0..pos) has new ids.  The workspace (M logits rows, M seen rows, K/V save rows for M-1 rows,
+ *                            the per-entry results) is the batch's own, allocated at its first call (a failed allocation fails the
+ *                            call before anything is written) and freed by nb200_batch_destroy.  device_ms (optional): CUDA-event
+ *                            time of the call.  NB200_EINVAL, with nothing written (every slot's cache, logits and seen set, every
+ *                            ids array): everything nb200_batch_next_greedy refuses, with the same messages; n_pos[i] == 0 or
+ *                            n_pos[i] > M; pos[i] + n_pos[i] > min(max_seq_len, block_size); an id >= vocab_size in ids[i][pos ..
+ *                            pos+n_pos) (and in ids[i][0..pos) when repetition_penalty[i] != 1).
  *   nb200_batch_read_logits / nb200_batch_read_kv  a slot's logits row, and its K / V cache rows as nb200_read_buffer gives them.
  *   nb200_batch_info         [0] M, [1] n_slots, [2] the attention kernel (encoded as nb200_config.reserved[4]), [3] 0.
  * A batch always runs the multi-kernel path's arithmetic, and a row's value depends neither on the other entries of its pass nor
@@ -248,6 +271,8 @@ int nb200_batch_next_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, c
 int nb200_batch_next_sampled(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t *const *ids, const uint32_t *pos,
                              const float *repetition_penalty, const float *temperature, const float *top_p, const float *coin,
                              uint32_t *next_tokens, uint32_t *top6 /* n x 6, optional */, float *device_ms);
+int nb200_batch_verify_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, uint32_t *const *ids, const uint32_t *pos,
+                              const uint32_t *n_pos, const float *repetition_penalty, uint32_t *n_accepted, float *device_ms);
 int nb200_batch_read_logits(nb200_batch *b, uint32_t slot, float *host_logits);
 int nb200_batch_read_kv(nb200_batch *b, uint32_t slot, int field /* NB200_F_KROW | NB200_F_VROW */, uint32_t layer, uint32_t pos,
                         float *dst, uint32_t count);

@@ -12,7 +12,8 @@
 // then the classifier (final rmsnorm, the slot's repetition penalty, logits row) and one argmax CTA per entry.
 // The residual / SwiGLU matvecs do not depend on the position and are prefill's own kernels.  There is no K-row pass: the
 // entries of a pass belong to different slots, so no entry reads a row another entry writes, and within an entry the
-// attention CTA that owns row pos writes it before reading it, as on the token path.
+// attention CTA that owns row pos writes it before reading it, as on the token path.  (A verify pass, at the end of this file,
+// has rows of one slot at consecutive positions and adds one.)
 #pragma once
 #include "prefill.cuh"
 
@@ -186,6 +187,126 @@ NB_K __global__ void __launch_bounds__(1024) k_verify_seen(const VerifySeenArgs 
     for (uint32_t i = threadIdx.x; i < a.V; i += 1024) row[i] = a.seen[i];
     __syncthreads();
     if (threadIdx.x < j) row[a.ids[threadIdx.x]] = 1;
+}
+
+// ---------------- batched verification (nb200_batch_verify_greedy) ----------------
+// A verify pass of a batch packs entries of 1 .. M rows: entry e runs the consumed id and its drafts at positions pos .. pos+n-1
+// of its slot, rows r0 .. r0+n-1 of the pass.  The QKV matvec and the attention kernels above take a per-row (slot, position),
+// so rows of one slot at consecutive positions need nothing new there; what is new is prefill's K-row pass with a per-row slot
+// (a row reads the K rows of its entry's earlier rows), the seen rows, and saving / accepting the rows past the accepted ones on
+// the device, so that a call of several passes never waits for the host.
+// The verify pass's own kernels are named k_vbatch_*, apart from the decode pass's k_batch_* set.
+
+// per entry of a pass (pass-local index e): its slot, first position, row count and first row
+struct BatchVerifyEntries { uint32_t slot[kPrefillMax], pos[kPrefillMax], n[kPrefillMax], r0[kPrefillMax]; };
+
+// K-row pass of a verify pass: krow_store (k_prefill_krow's body) for row r of the pass at (slot[r], pos[r]).  One warp per
+// (kv head, row).
+struct BatchKrowArgs {
+    const float *kraw;                      // [R][kv_dim]
+    float *kc;                              // K cache of this layer in slot 0; slot s starts slot_elems floats further
+    size_t slot_elems;
+    const float *knorm, *rope_cos, *rope_sin;
+    BatchPass bp;                           // pen unused
+    uint32_t fast;
+    Dims d;
+};
+NB_K __global__ void __launch_bounds__(32) k_vbatch_krow(const BatchKrowArgs a) {
+    __shared__ __align__(16) float h[512];
+    pdl_launch_dependents();
+    pdl_wait();
+    const Dims &d = a.d;
+    const uint32_t hd = d.hd, g = blockIdx.x, r = blockIdx.y, pos = a.bp.pos[r];
+    float *kc = a.kc + (size_t)a.bp.slot[r] * a.slot_elems;
+    krow_store(a.kraw + (size_t)r * d.kv_dim + (size_t)g * hd, kc + ((size_t)g * d.max_seq + pos) * hd, a.knorm,
+               a.rope_cos + (size_t)pos * (hd / 2), a.rope_sin + (size_t)pos * (hd / 2), a.fast, d, h, threadIdx.x & 31);
+}
+
+// Seen rows of a verify pass, one CTA per row: row r is its slot's seen set (ids[0..pos), brought up to date by the host) plus
+// the ids its entry's earlier rows consume (ids[first[r] .. r) of the pass), so the classifier of row r penalises exactly what
+// nb200_next_greedy at pos[r] would.  Rows of entries at penalty 1 are not read by the classifier and are left alone.
+struct BatchSeenArgs {
+    uint8_t *rows;                          // [M][V]
+    const uint8_t *seen;                    // the batch's seen sets [n_slots][V]
+    const uint32_t *ids;                    // the ids the pass's rows consume
+    BatchPass bp;
+    uint32_t first[kPrefillMax];            // first row of row r's entry
+    uint32_t V;
+};
+NB_K __global__ void __launch_bounds__(1024) k_vbatch_seen(const BatchSeenArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const uint32_t r = blockIdx.x;
+    if (a.bp.pen[r] == 1.0f) return;
+    uint8_t *row = a.rows + (size_t)r * a.V;
+    const uint8_t *src = a.seen + (size_t)a.bp.slot[r] * a.V;
+    for (uint32_t i = threadIdx.x; i < a.V; i += 1024) row[i] = src[i];
+    __syncthreads();
+    if (threadIdx.x >= a.first[r] && threadIdx.x < r) row[a.ids[threadIdx.x]] = 1;
+}
+
+// Before a verify pass: the K and V rows its drafted rows will overwrite.  Row r (bit r of `drafted`: not the first row of its
+// entry) at (slot[r], pos[r]) goes to save row r-1 (entries own disjoint rows, so M-1 save rows suffice), for every kv head of
+// layer blockIdx.y.  Save layout [L][KV][M-1][hd].
+struct BatchSaveArgs {
+    const float *kc, *vc;                   // the batch's caches, slot 0
+    float *ksave, *vsave;
+    size_t slot_elems;
+    BatchPass bp;
+    uint32_t drafted, M;
+    Dims d;
+};
+NB_K __global__ void __launch_bounds__(256) k_vbatch_save(const BatchSaveArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const Dims &d = a.d;
+    const uint32_t r = blockIdx.x, l = blockIdx.y, hd = d.hd;
+    if (!((a.drafted >> r) & 1u)) return;
+    const size_t off = (size_t)a.bp.slot[r] * a.slot_elems + ((size_t)l * d.KV * d.max_seq + a.bp.pos[r]) * hd;
+    const size_t sv = ((size_t)l * d.KV * (a.M - 1) + (r - 1)) * hd;
+    for (uint32_t i = threadIdx.x; i < d.KV * hd; i += 256) {
+        const uint32_t g = i / hd, c = i % hd;
+        a.ksave[sv + (size_t)g * (a.M - 1) * hd + c] = a.kc[off + (size_t)g * d.max_seq * hd + c];
+        a.vsave[sv + (size_t)g * (a.M - 1) * hd + c] = a.vc[off + (size_t)g * d.max_seq * hd + c];
+    }
+}
+
+// After the argmax: per entry (blockIdx.x), a = the largest count whose greedy ids next[r0 .. r0+a) equal the drafts the next
+// rows consumed, res[2e] = a and res[2e+1] = g_a; the slot's logits row becomes row r0+a of the pass, and the saved rows
+// pos+a+1 .. pos+n-1 go back.  The copies are spread over blockIdx.y; every CTA of the entry finds the same a.
+struct BatchAcceptArgs {
+    const uint32_t *next, *ids;             // the pass's greedy ids and the ids its rows consumed
+    const float *ws_logits;                 // [M][V] the pass's logits rows
+    float *logits;                          // the batch's logits rows [n_slots][V]
+    float *kc, *vc;
+    const float *ksave, *vsave;
+    size_t slot_elems;
+    uint32_t *res;                          // [2 * entries of the pass]
+    BatchVerifyEntries en;
+    uint32_t M;
+    Dims d;
+};
+NB_K __global__ void __launch_bounds__(1024) k_vbatch_accept(const BatchAcceptArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const Dims &d = a.d;
+    const uint32_t e = blockIdx.x, r0 = a.en.r0[e], n = a.en.n[e], slot = a.en.slot[e], pos = a.en.pos[e], hd = d.hd;
+    uint32_t acc = 0;
+    while (acc + 1 < n && a.next[r0 + acc] == a.ids[r0 + acc + 1]) acc++;
+    if (blockIdx.y == 0 && threadIdx.x == 0) { a.res[2 * e] = acc; a.res[2 * e + 1] = a.next[r0 + acc]; }
+    const uint32_t tid = blockIdx.y * 1024 + threadIdx.x, stride = gridDim.y * 1024;
+    const float *src = a.ws_logits + (size_t)(r0 + acc) * d.V;
+    float *dst = a.logits + (size_t)slot * d.V;
+    for (uint32_t i = tid; i < d.V; i += stride) dst[i] = src[i];
+    // rows r0+acc+1 .. r0+n-1 (save rows r-1) back to positions pos+acc+1 .. pos+n-1, every layer and kv head
+    const uint32_t rows = n - 1 - acc, per_row = d.L * d.KV * hd;
+    for (uint32_t i = tid; i < rows * per_row; i += stride) {
+        const uint32_t j = i / per_row, rest = i % per_row, lg = rest / hd, c = rest % hd;     // lg = layer * KV + kv head
+        const size_t sv = ((size_t)lg * (a.M - 1) + (r0 + acc + j)) * hd + c;
+        const size_t cv = (size_t)slot * a.slot_elems + ((size_t)lg * d.max_seq + pos + acc + 1 + j) * hd + c;
+        a.kc[cv] = a.ksave[sv];
+        a.vc[cv] = a.vsave[sv];
+    }
 }
 
 }  // namespace nb

@@ -1630,6 +1630,15 @@ struct nb200_batch {
     void *samp_ws = nullptr; size_t samp_cub = 0;
     uint32_t *res_dev = nullptr, *res_host = nullptr;         // [n_slots][16]
     std::vector<SampleRows> samp_pass;                        // [max_pass]
+    // verification (nb200_batch_verify_greedy), allocated at the first call: M logits rows and M seen rows of a pass, its M greedy
+    // ids, the ids the rows of every pass of a call consume, the K / V rows a pass may overwrite past the accepted ones
+    // ([L][KV][M-1][hd] each), the per-entry results {a, g_a} and their pinned host copy
+    struct Verify {
+        float *logits = nullptr;
+        uint8_t *seen = nullptr;
+        uint32_t *next = nullptr, *ids = nullptr, *res = nullptr, *res_host = nullptr;
+        float *ksave = nullptr, *vsave = nullptr;
+    } ver;
     LayerBufs buf;                            // M positions
     std::vector<std::vector<uint32_t>> mirror;
     std::vector<char> mirror_valid;
@@ -1725,6 +1734,7 @@ void nb200_batch_destroy(nb200_batch *b) {
     if (b->ids_pass_host) cudaFreeHost(b->ids_pass_host);
     if (b->next_host) cudaFreeHost(b->next_host);
     if (b->res_host) cudaFreeHost(b->res_host);
+    if (b->ver.res_host) cudaFreeHost(b->ver.res_host);
     delete b;
 }
 
@@ -1887,9 +1897,165 @@ int batch_step(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t
     return 0;
 }
 
+// The batch's verify workspace (Verify), allocated at the first call; a failed allocation fails the call before anything is written.
+int batch_verify_setup(nb200_batch *b) {
+    if (b->ver.res_host) return 0;
+    const Dims &d = b->e->d;
+    const uint32_t M = b->M;
+    const size_t save = (size_t)d.L * d.KV * (M - 1) * d.hd * 4;
+    nb200_batch::Verify v;
+    DMV(b->allocs, v.logits, (size_t)M * d.V * 4); DMV(b->allocs, v.seen, (size_t)M * d.V); DMV(b->allocs, v.next, (size_t)M * 4);
+    DMV(b->allocs, v.ids, (size_t)b->n_slots * M * 4); DMV(b->allocs, v.res, (size_t)b->n_slots * 2 * 4);
+    DMV(b->allocs, v.ksave, save); DMV(b->allocs, v.vsave, save);
+    CK(cudaHostAlloc(&v.res_host, (size_t)b->n_slots * 2 * 4, cudaHostAllocDefault));
+    b->ver = v;
+    return 0;
+}
+
+// One verify pass of a batch, R rows packed from the entries en (the ids its rows consume at ids on the device): save -> seen
+// rows -> chunk (with the K-row pass) -> classifier -> argmax -> accept, results of the pass's entries at res[2e ..].
+// rows: row r at (slot, pos) of its entry, with its penalty; first[r]: the first row of r's entry; drafted: bit r where r is not.
+int run_batch_verify_pass(nb200_batch *b, const BatchPass &rows, const uint32_t *first, uint32_t drafted, const BatchVerifyEntries &en,
+                          uint32_t n_ent, uint32_t R, bool penalised, const uint32_t *ids, uint32_t *res) {
+    nb200_engine *e = b->e;
+    const Dims &d = e->d;
+    const LayerBufs &buf = b->buf;
+    const auto &v = b->ver;
+    const size_t kvl = (size_t)d.KV * d.max_seq * d.hd;
+    const AttnChoice ac = pick_attn(e);
+    int r;
+    if (drafted) {
+        BatchSaveArgs sa{b->kc, b->vc, v.ksave, v.vsave, b->slot_elems, rows, drafted, b->M, d};
+        if ((r = launch<BatchSaveArgs>(e, k_vbatch_save, dim3(R, d.L), dim3(256), 0, sa))) return r;
+    }
+    if (penalised) {
+        BatchSeenArgs sa{};
+        sa.rows = v.seen; sa.seen = b->seen; sa.ids = ids; sa.bp = rows; sa.V = d.V;
+        for (uint32_t j = 0; j < R; j++) sa.first[j] = first[j];
+        if ((r = launch<BatchSeenArgs>(e, k_vbatch_seen, dim3(R), dim3(1024), 0, sa))) return r;
+    }
+    {
+        PrefillEmbedArgs a{e->emb.w, e->emb.aux, buf.x, ids, d};
+        if ((r = launch<PrefillEmbedArgs>(e, k_prefill_embed, dim3(R), dim3(256), 0, a))) return r;
+    }
+    for (uint32_t l = 0; l < d.L; l++) {
+        BatchMvArgs a{};
+        a.mv.m = R;
+        a.mv.src = buf.x; a.mv.src_stride = d.E; a.mv.gain = e->norm_attn + (size_t)l * d.E;
+        a.mv.out = buf.q; a.mv.out_stride = d.q_dim; a.mv.out_k = buf.kraw; a.mv.k_stride = d.kv_dim;
+        a.bp = rows; a.vc = b->vc + l * kvl; a.slot_elems = b->slot_elems;
+        if ((r = run_batch_matvec(e, EPI_QKV, e->qkv[l], a))) return r;
+
+        BatchAttnArgs ba{};
+        attn_args(e, buf, b->kc, b->vc, l, ba.pa.at, ba.pa.ex);
+        ba.bp = rows; ba.slot_elems = b->slot_elems;
+        BatchKrowArgs kr{buf.kraw, ba.pa.at.kc, b->slot_elems, ba.pa.at.knorm, e->rope_cos, e->rope_sin, rows, ac.kvm ? 1u : 0u, d};
+        if ((r = launch<BatchKrowArgs>(e, k_vbatch_krow, dim3(d.KV, R), dim3(32), 0, kr))) return r;
+        const dim3 grid = d.exact ? dim3(d.H, R) : dim3(e->nsplit_max, d.KV, R);
+        if ((r = launch<BatchAttnArgs>(e, ac.batch, grid, dim3(ac.threads), ac.smem, ba))) return r;
+
+        if ((r = run_chunk_ffn(e, buf, l, 0, R))) return r;
+    }
+    BatchPass cls = rows;                   // row r's classifier writes logits row r and reads seen row r of the workspace
+    for (uint32_t j = 0; j < R; j++) cls.slot[j] = j;
+    BatchMvArgs a{};
+    a.mv.m = R;
+    a.mv.src = buf.x; a.mv.src_stride = d.E; a.mv.gain = e->norm_final;
+    a.bp = cls; a.logits = v.logits; a.seen = v.seen;
+    if ((r = run_batch_matvec(e, EPI_CLS, e->cls, a))) return r;
+    BatchArgmaxArgs am{v.logits, cls, v.next, d.V};
+    if ((r = launch<BatchArgmaxArgs>(e, k_batch_argmax, dim3(R), dim3(1024), 0, am))) return r;
+    BatchAcceptArgs ak{v.next, ids, v.logits, b->logits, b->kc, b->vc, v.ksave, v.vsave, b->slot_elems, res, en, b->M, d};
+    const uint32_t gy = 1 + d.V / 16384;
+    return launch<BatchAcceptArgs>(e, k_vbatch_accept, dim3(n_ent, gy < 32 ? gy : 32), dim3(1024), 0, ak);
+}
+
+// nb200_batch_verify_greedy: every check, the packing, then the passes and one synchronise at the end
+int batch_verify(nb200_batch *b, uint32_t n, const uint32_t *slots, uint32_t *const *ids, const uint32_t *pos, const uint32_t *n_pos,
+                 const float *repetition_penalty, uint32_t *n_accepted, float *device_ms) {
+    int r;
+    if ((r = batch_usable(b))) return r;
+    nb200_engine *e = b->e;
+    const Dims &d = e->d;
+    const uint32_t M = b->M;
+    if (!slots || !ids || !pos || !n_pos || !repetition_penalty || !n_accepted) return fail(NB200_EINVAL, "null argument");
+    if (n == 0) return fail(NB200_EINVAL, "no entries");
+    // every check before anything is written
+    std::vector<char> used(b->n_slots, 0);
+    const uint32_t lim = pos_limit(d);
+    for (uint32_t i = 0; i < n; i++) {
+        if (slots[i] >= b->n_slots) return fail(NB200_EINVAL, "entry %u: slot %u of a batch of %u", i, slots[i], b->n_slots);
+        if (used[slots[i]]) return fail(NB200_EINVAL, "entry %u: slot %u appears twice in one call", i, slots[i]);
+        used[slots[i]] = 1;
+        if (!ids[i]) return fail(NB200_EINVAL, "entry %u: null ids", i);
+        if (n_pos[i] == 0 || n_pos[i] > M)
+            return fail(NB200_EINVAL, "entry %u: verify of %u positions: a pass verifies 1 .. M = %u positions", i, n_pos[i], M);
+        if (pos[i] >= lim || n_pos[i] > lim - pos[i])
+            return fail(NB200_EINVAL, "entry %u: verify of %u positions from %u: past min(max_seq_len, block_size) = %u", i, n_pos[i], pos[i], lim);
+        const uint32_t upto = (repetition_penalty[i] != 1.0f) ? 0 : pos[i];      // the penalty reads ids[0..pos)
+        for (uint32_t p = upto; p < pos[i] + n_pos[i]; p++)
+            if (ids[i][p] >= d.V) return fail(NB200_EINVAL, "entry %u: id %u at position %u out of range", i, ids[i][p], p);
+    }
+    CK(cudaSetDevice(e->device));
+    if ((r = batch_verify_setup(b))) return r;
+    // the packing: entries in call order, a new pass when the next entry does not fit in the rows left
+    struct Pass { BatchPass rows{}; uint32_t first[kPrefillMax] = {}; BatchVerifyEntries en{}; uint32_t R = 0, n_ent = 0, drafted = 0, row0 = 0, ent0 = 0; bool pen = false; };
+    std::vector<Pass> passes;
+    std::vector<uint32_t> ids_rows;         // the ids every row of the call consumes, pass after pass
+    for (uint32_t i = 0; i < n; i++) {
+        if (passes.empty() || passes.back().R + n_pos[i] > M) {
+            passes.emplace_back();
+            passes.back().row0 = (uint32_t)ids_rows.size(); passes.back().ent0 = i;
+        }
+        Pass &ps = passes.back();
+        const uint32_t r0 = ps.R, k = ps.n_ent++;
+        ps.en.slot[k] = slots[i]; ps.en.pos[k] = pos[i]; ps.en.n[k] = n_pos[i]; ps.en.r0[k] = r0;
+        for (uint32_t j = 0; j < n_pos[i]; j++) {
+            ps.rows.slot[r0 + j] = slots[i]; ps.rows.pos[r0 + j] = pos[i] + j; ps.rows.pen[r0 + j] = repetition_penalty[i];
+            ps.first[r0 + j] = r0;
+            if (j) ps.drafted |= 1u << (r0 + j);
+            ids_rows.push_back(ids[i][pos[i] + j]);
+        }
+        ps.R += n_pos[i];
+        ps.pen |= repetition_penalty[i] != 1.0f;
+    }
+    struct Events { cudaEvent_t ev[2] = {nullptr, nullptr}; ~Events() { for (auto x : ev) if (x) cudaEventDestroy(x); } } evs;
+    for (auto &x : evs.ev) CK(cudaEventCreate(&x));
+    CK(cudaEventRecord(evs.ev[0], e->stream));
+    for (uint32_t i = 0; i < n; i++) {
+        if (repetition_penalty[i] == 1.0f) continue;       // x / 1.0f == x: the classifier skips the lookup, as nb200_next_greedy
+        const uint32_t s = slots[i];
+        bool valid = b->mirror_valid[s] != 0;
+        r = sync_seen_set(e, b->seen + (size_t)s * d.V, b->ids + (size_t)s * d.max_seq, b->mirror[s], valid, ids[i], pos[i]);
+        b->mirror_valid[s] = valid ? 1 : 0;
+        if (r) return r;
+    }
+    CK(cudaMemcpyAsync(b->ver.ids, ids_rows.data(), ids_rows.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    for (const Pass &ps : passes)
+        if ((r = run_batch_verify_pass(b, ps.rows, ps.first, ps.drafted, ps.en, ps.n_ent, ps.R, ps.pen, b->ver.ids + ps.row0,
+                                       b->ver.res + 2 * ps.ent0))) return r;
+    CK(cudaEventRecord(evs.ev[1], e->stream));
+    CK(cudaMemcpyAsync(b->ver.res_host, b->ver.res, (size_t)n * 2 * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t a = b->ver.res_host[2 * i];
+        n_accepted[i] = a;
+        ids[i][pos[i] + a + 1] = b->ver.res_host[2 * i + 1];
+    }
+    float ms = 0.0f;
+    CK(cudaEventElapsedTime(&ms, evs.ev[0], evs.ev[1]));
+    if (device_ms) *device_ms = ms;
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
+
+int nb200_batch_verify_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, uint32_t *const *ids, const uint32_t *pos,
+                              const uint32_t *n_pos, const float *repetition_penalty, uint32_t *n_accepted, float *device_ms) {
+    return batch_verify(b, n, slots, ids, pos, n_pos, repetition_penalty, n_accepted, device_ms);
+}
 
 int nb200_batch_next_greedy(nb200_batch *b, uint32_t n, const uint32_t *slots, const uint32_t *const *ids, const uint32_t *pos,
                             const float *repetition_penalty, uint32_t *next_tokens, float *device_ms) {

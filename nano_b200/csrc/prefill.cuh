@@ -194,6 +194,31 @@ struct PrefillKrowArgs {
     uint32_t pos0, fast;
     Dims d;
 };
+// One K row (one warp, lane = threadIdx.x & 31): kr is the raw k of the kv head, dst its cache row, cr / ci the RoPE row of its
+// position, h a staging row in shared memory (fast = 0).  The body of k_prefill_krow and of the batch's k_vbatch_krow (batch.cuh).
+__device__ __forceinline__ void krow_store(const float *kr, float *dst, const float *knorm, const float *cr, const float *ci,
+                                           uint32_t fast, const Dims &d, float *h, int lane) {
+    const uint32_t hd = d.hd;
+    if (fast) {
+        uint32_t lpr = 1; while (lpr * 4 < hd) lpr <<= 1;
+        const uint32_t sub = lane / lpr, col = (lane % lpr) * 4;
+        const bool colon = col < hd;
+        float4 kk0 = make_float4(0, 0, 0, 0), gk = make_float4(0, 0, 0, 0);
+        if (colon) {
+            kk0 = __ldcg(reinterpret_cast<const float4 *>(kr + col));
+            if (d.arch == 3u) gk = *reinterpret_cast<const float4 *>(knorm + col);
+        }
+        const RopeTab rt = rope_tab_load(cr, ci, d, col, colon);
+        const float4 kk = norm_rope_apply(kk0, gk, rt, d, lpr, col, colon);     // every lane group of the warp (shuffles)
+        if (sub == 0 && colon) *reinterpret_cast<float4 *>(dst + col) = kk;
+    } else {
+        for (uint32_t i = lane; i < hd; i += 32) h[i] = __ldcg(kr + i);
+        __syncwarp();
+        head_norm_rope(h, knorm, cr, ci, d, d.exact != 0);
+        for (uint32_t i = lane; i < hd; i += 32) dst[i] = h[i];
+    }
+}
+
 NB_K __global__ void __launch_bounds__(32) k_prefill_krow(const PrefillKrowArgs a) {
     __shared__ __align__(16) float h[512];
     pdl_launch_dependents();
@@ -204,24 +229,7 @@ NB_K __global__ void __launch_bounds__(32) k_prefill_krow(const PrefillKrowArgs 
     const float *kr = a.kraw + (size_t)p * d.kv_dim + (size_t)g * hd;
     const float *cr = a.rope_cos + (size_t)pos * (hd / 2), *ci = a.rope_sin + (size_t)pos * (hd / 2);
     float *dst = a.kc + ((size_t)g * d.max_seq + pos) * hd;
-    if (a.fast) {
-        uint32_t lpr = 1; while (lpr * 4 < hd) lpr <<= 1;
-        const uint32_t sub = lane / lpr, col = (lane % lpr) * 4;
-        const bool colon = col < hd;
-        float4 kk0 = make_float4(0, 0, 0, 0), gk = make_float4(0, 0, 0, 0);
-        if (colon) {
-            kk0 = __ldcg(reinterpret_cast<const float4 *>(kr + col));
-            if (d.arch == 3u) gk = *reinterpret_cast<const float4 *>(a.knorm + col);
-        }
-        const RopeTab rt = rope_tab_load(cr, ci, d, col, colon);
-        const float4 kk = norm_rope_apply(kk0, gk, rt, d, lpr, col, colon);     // every lane group of the warp (shuffles)
-        if (sub == 0 && colon) *reinterpret_cast<float4 *>(dst + col) = kk;
-    } else {
-        for (uint32_t i = lane; i < hd; i += 32) h[i] = __ldcg(kr + i);
-        __syncwarp();
-        head_norm_rope(h, a.knorm, cr, ci, d, d.exact != 0);
-        for (uint32_t i = lane; i < hd; i += 32) dst[i] = h[i];
-    }
+    krow_store(kr, dst, a.knorm, cr, ci, a.fast, d, h, lane);
 }
 
 // Attention of every position of the chunk: blockIdx.z = position p, which attends to rows [0, pos0 + p] through the token

@@ -33,7 +33,7 @@ EXPORTS = [
     "nb200_lora_load", "nb200_lora_enable", "nb200_lora_unload",
     "nb200_engine_create_tp", "nb200_tp_export", "nb200_tp_attach_ipc", "nb200_tp_attach_local",
     "nb200_batch_create", "nb200_batch_destroy", "nb200_batch_prefill", "nb200_batch_next_greedy", "nb200_batch_next_sampled",
-    "nb200_batch_read_logits", "nb200_batch_read_kv", "nb200_batch_info",
+    "nb200_batch_verify_greedy", "nb200_batch_read_logits", "nb200_batch_read_kv", "nb200_batch_info",
 ]
 
 
@@ -104,6 +104,7 @@ def lib():
         L.nb200_batch_next_greedy.argtypes = [C.c_void_p, C.c_uint32, u32p, C.POINTER(u32p), u32p, f32p, u32p, f32p]
         L.nb200_batch_next_sampled.argtypes = [C.c_void_p, C.c_uint32, u32p, C.POINTER(u32p), u32p, f32p, f32p, f32p, f32p, u32p, u32p,
                                                f32p]
+        L.nb200_batch_verify_greedy.argtypes = [C.c_void_p, C.c_uint32, u32p, C.POINTER(u32p), u32p, u32p, f32p, u32p, f32p]
         L.nb200_batch_read_logits.argtypes = [C.c_void_p, C.c_uint32, f32p]
         L.nb200_batch_read_kv.argtypes = [C.c_void_p, C.c_uint32, C.c_int, C.c_uint32, C.c_uint32, f32p, C.c_uint32]
         L.nb200_batch_info.argtypes = [C.c_void_p, u32p]
@@ -349,7 +350,7 @@ class Batch:
         self.engine = engine
         self.h = C.c_void_p()
         _check(lib().nb200_batch_create(engine.h, int(n_slots), C.byref(self.h)))
-        self.device_ms = 0.0        # device time of the last next_greedy / next_sampled
+        self.device_ms = 0.0        # device time of the last next_greedy / next_sampled / verify_greedy
 
     def info(self) -> dict:
         """{"chunk": positions per pass M, "slots": n_slots, "attention": the attention kernel, named as Engine.kernels()}"""
@@ -393,6 +394,24 @@ class Batch:
                                               _p(c, f32p), _p(out, u32p), _p(six, u32p), C.byref(ms)))
         self.device_ms = float(ms.value)
         return out.tolist(), six.tolist()
+
+    def verify_greedy(self, slots, ids, pos, n_pos, penalties) -> list:
+        """Entry i is Engine.verify_greedy(ids[i], pos[i], n_pos[i], penalties[i]) in slot slots[i]: returns the accepted counts
+        and writes each entry's greedy id at pos+a into ids[i][pos+a+1] in place (ids[i]: uint32, at least pos+n_pos+1
+        entries).  The device time of the call is left in self.device_ms."""
+        n = len(slots)
+        assert len(ids) == len(pos) == len(n_pos) == len(penalties) == n
+        for a, p, k in zip(ids, pos, n_pos):
+            assert a.dtype == np.uint32 and a.flags.c_contiguous and a.size >= p + k + 1
+        ptrs = (u32p * n)(*[_p(a, u32p) for a in ids])
+        s = np.asarray(slots, np.uint32); p = np.asarray(pos, np.uint32); k = np.asarray(n_pos, np.uint32)
+        pen = np.asarray(penalties, np.float32)
+        acc = np.zeros(n, np.uint32)
+        ms = C.c_float(0)
+        _check(lib().nb200_batch_verify_greedy(self.h, n, _p(s, u32p), ptrs, _p(p, u32p), _p(k, u32p), _p(pen, f32p), _p(acc, u32p),
+                                               C.byref(ms)))
+        self.device_ms = float(ms.value)
+        return acc.tolist()
 
     def logits(self, slot: int) -> np.ndarray:
         out = np.empty(self.engine.vocab, dtype=np.float32)
