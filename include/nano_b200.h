@@ -63,7 +63,7 @@ typedef struct nb200_config {
     uint32_t block_size, vocab_size, n_layer, n_embd, n_head, n_kv_head, n_hidden, tied, head_dim;
     uint32_t q_dim, kv_dim, max_seq_len;
     uint32_t tp_rank, tp_size;
-    uint32_t reserved[7];   /* [0] execution path: 4 | CTAs << 8 streaming kernel on a grid of that many CTAs, 1 CUDA graph, 0 direct launches; [1], [2] creation-time calibration:
+    uint32_t reserved[7];   /* [0] execution path: 4 | CTAs << 8 | C << 24 streaming kernel on a grid of that many CTAs, launched in clusters of C CTAs (0: plain launch), 1 CUDA graph, 0 direct launches; [1], [2] creation-time calibration:
                                us per token of the streaming kernel / of the multi-kernel graph (0 = the choice was not measured);
                                multi-kernel path, recorded when a kernel is launched or captured into the graph:
                                [3] matvec variants used since creation, bit 3 * epilogue + {0: RB 1, 1: RB 2, 2: RB 4} with the

@@ -35,6 +35,7 @@ def _newer(target: str, sources) -> bool:
 UNITS = {
     "engine.cu": ["kernels.cuh", "prefill.cuh", "batch.cuh", "expf_ref.cuh", "stream_args.h", "stream_host.h", "sample_host.h", "../../include/nano_b200.h"],
     "stream.cu": ["kernels.cuh", "expf_ref.cuh", "stream_args.h", "stream_host.h", "stream.cuh"],
+    "stream_cl.cu": ["kernels.cuh", "expf_ref.cuh", "stream_args.h", "stream_host.h", "stream.cuh"],
     "sample.cu": ["kernels.cuh", "expf_ref.cuh", "sample_host.h"],
 }
 
@@ -66,10 +67,12 @@ def build_trace_variant() -> str:
     """Developer build of the streaming kernel with its fine cycle stamps compiled in (-DNB200_FINE_TRACE; they cost ~200
     cycles each, so the product library never carries them).  Loaded by tools/gpu_trace.py through NB200_ENGINE_SO."""
     build_engine()
-    obj = os.path.join(LIB, "stream_trace.o")
-    subprocess.run([NVCC, *GENCODE, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
-                    "-DNB200_FINE_TRACE", "-c", os.path.join(CSRC, "stream.cu"), "-o", obj], check=True)
-    objs = [os.path.join(LIB, u[:-3] + ".o") for u in UNITS if u != "stream.cu"] + [obj]
+    traced = ("stream.cu", "stream_cl.cu")
+    procs = [subprocess.Popen([NVCC, *GENCODE, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-DNB200_FINE_TRACE",
+                               "-c", os.path.join(CSRC, u), "-o", os.path.join(LIB, u[:-3] + "_trace.o")]) for u in traced]
+    if any(p.wait() != 0 for p in procs):
+        raise RuntimeError("nvcc failed for the trace build")
+    objs = [os.path.join(LIB, u[:-3] + ".o") for u in UNITS if u not in traced] + [os.path.join(LIB, u[:-3] + "_trace.o") for u in traced]
     subprocess.run([NVCC, *GENCODE, "-shared", "-o", TRACE_SO] + objs, check=True)
     return TRACE_SO
 

@@ -114,6 +114,11 @@ struct nb200_engine {
     float calib_ms[2] = {0.0f, 0.0f};      // ms per token of {streaming, multi-kernel} measured by calibrate_paths (0 = not calibrated)
     bool use_stream = false; const void *st_kern = nullptr; StreamArgs sa{}; uint32_t st_smem = 0, st_grid = 0;
     bool st_width_fixed = false;                                 // NB200_STREAM_WIDTH chose st_grid (no width calibration)
+    // cluster launch (stream.cuh st_item): kernels of both launches, co-resident clusters of kStCluster CTAs (0: the shape or the
+    // GPU does not allow the cluster launch), whether it was forced (NB200_STREAM_CLUSTER), and the launch st_layout picked
+    const void *st_kern_plain = nullptr, *st_kern_cl = nullptr;
+    uint32_t st_max_clusters = 0; bool st_cl_forced = false;
+    uint32_t st_cl = 0;                                          // kStCluster when st_kern is the cluster kernel, else 0
     uint32_t *st_err_host = nullptr, *st_err_dev = nullptr;      // mapped pinned word: the code a device-side spin recorded before trapping
     uint32_t st_epoch = 0;                                       // exchange epochs handed out so far (stream.cuh)
     void *samp_ws = nullptr; size_t samp_cub = 0; uint32_t *samp_host = nullptr;       // device-side sampler workspace (sample.cu), pinned result
@@ -604,7 +609,23 @@ int launch_stream(nb200_engine *e, uint32_t n_steps) {
     e->st_epoch += n_steps * 5u * e->d.L;
     CK(cudaMemsetAsync(e->bar, 0, sizeof(unsigned int), e->stream));
     void *params[] = {&g};
-    CK(cudaLaunchCooperativeKernel(e->st_kern, dim3(e->st_grid), dim3(kThreads), params, e->st_smem, e->stream));
+    if (e->st_cl) {
+        // Clusters of st_cl CTAs.  The kernel's only grid-wide wait is its own counter barrier, so what the launch must
+        // guarantee is that every CTA is resident at once: setup_stream checked that W / st_cl clusters fit side by side
+        // (cudaOccupancyMaxActiveClusters), and the cooperative attribute makes the runtime refuse the launch otherwise.
+        // A refused launch is an error, never a launch without the guarantee.
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(e->st_grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = e->st_smem; cfg.stream = e->stream;
+        cudaLaunchAttribute attr[2];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = e->st_cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        attr[1].id = cudaLaunchAttributeCooperative;
+        attr[1].val.cooperative = 1;
+        cfg.attrs = attr; cfg.numAttrs = 2;
+        CK(cudaLaunchKernelExC(&cfg, e->st_kern, params));
+    } else {
+        CK(cudaLaunchCooperativeKernel(e->st_kern, dim3(e->st_grid), dim3(kThreads), params, e->st_smem, e->stream));
+    }
     e->launches++;
     return 0;
 }
@@ -695,21 +716,39 @@ uint32_t env_u32(const char *name, uint32_t dflt) { const char *s = getenv(name)
 //    KV * nsplit at the longest range (nsplit <= the split count st_attn_plan starts from, monotonic in the range).
 //  - Every CTA merges the per-CTA classifier partials by (value, lowest index): the same id for any W.
 //  - A CTA keeps at most kStOwnMax residual rows.
+//  - Cluster launch (st_cl_width_ok): kv head h runs on cluster h, its split sp on the cluster's CTA of rank sp.  So W is a multiple
+//    of kStCluster, at least KV clusters, and at most the clusters that are resident at once.
+// Attention split count at the longest range (max_seq: non-causal steps attend over all of it), the most any step uses
+uint32_t st_splits_max(const Dims &d, uint32_t chunk_target, uint32_t nsplit_max) {
+    uint32_t ns = (d.max_seq + chunk_target - 1) / chunk_target;
+    if (ns < 1) ns = 1;
+    if (ns > nsplit_max) ns = nsplit_max;
+    return ns;
+}
 uint32_t st_width_min(const nb200_engine *e) {
     const Dims &d = e->d;
     const StreamArgs &g = e->sa;
-    uint32_t ns = (d.max_seq + g.chunk_target - 1) / g.chunk_target;      // non-causal steps attend over max_seq rows
-    if (ns < 1) ns = 1;
-    if (ns > g.nsplit_max) ns = g.nsplit_max;
-    uint32_t w = d.KV * ns;
+    uint32_t w = d.KV * st_splits_max(d, g.chunk_target, g.nsplit_max);
     const uint32_t own = (d.E + kStOwnMax - 1) / kStOwnMax;
     return w > own ? w : own;
 }
 
+bool st_cl_width_ok(const nb200_engine *e, uint32_t W) {
+    const uint32_t C = (uint32_t)kStCluster;
+    return e->st_max_clusters && W % C == 0 && W >= e->d.KV * C && W / C <= e->st_max_clusters && W >= st_width_min(e) && W <= (uint32_t)e->num_sms;
+}
+
 // Per-CTA row slices, tiles and the tile-ordered stream copy of the weights for a grid of W CTAs (replaces an earlier copy).
+// Where the cluster launch is allowed and W is a legal width for it, the engine runs the cluster kernel.
 int st_layout(nb200_engine *e, uint32_t W) {
     const Dims &d = e->d;
     StreamArgs &g = e->sa;
+    const bool cl = st_cl_width_ok(e, W);
+    if (e->st_cl_forced && !cl)
+        return fail(NB200_EINVAL, "NB200_STREAM_CLUSTER=%d: %u CTAs is not a multiple of %d of at least %u and at most %u CTAs", kStCluster, W,
+                    kStCluster, d.KV * (uint32_t)kStCluster, e->st_max_clusters * (uint32_t)kStCluster);
+    e->st_cl = cl ? (uint32_t)kStCluster : 0u;
+    e->st_kern = cl ? e->st_kern_cl : e->st_kern_plain;
     if (g.stream) {
         for (auto it = e->allocs.begin(); it != e->allocs.end(); ++it) if (*it == (const void *)g.stream) { e->allocs.erase(it); break; }
         CK(cudaFree((void *)g.stream));
@@ -777,7 +816,7 @@ int st_layout(nb200_engine *e, uint32_t W) {
 int setup_stream(nb200_engine *e) {
     const Dims &d = e->d;
     if (d.exact || e->tp_size > 1) return 0;
-    StreamKern k = pick_stream(d);
+    StreamKern k = pick_stream(d, false);
     if (!k) return 0;
     uint32_t maxn = d.E; if (d.q_dim > maxn) maxn = d.q_dim; if (d.F > maxn) maxn = d.F;
     if (maxn > st_prep_max_n(d.quant, d.gs)) return 0;
@@ -787,6 +826,24 @@ int setup_stream(nb200_engine *e) {
     if (!coop) return 0;
     const uint32_t NC = (uint32_t)e->num_sms;
     if (d.KV > NC || (d.E + NC - 1) / NC > (uint32_t)kStOwnMax) return 0;
+    const uint32_t nsplit_max = e->nsplit_max;          // num_sms / kv heads (<= 64), as the multi-kernel path
+    // The cluster launch (stream.cuh st_item) takes shapes whose kv heads each fit one cluster at every range: at most kStCluster
+    // splits at max_seq (the split count st_attn_plan starts from is monotonic in the range), and KV clusters on the GPU.
+    // NB200_STREAM_CLUSTER=0 forbids it, =kStCluster requires it (NB200_EINVAL where it cannot run); unset: wherever it can.
+    const char *cl_env = getenv("NB200_STREAM_CLUSTER");
+    const bool cl_set = cl_env && *cl_env;
+    const uint32_t cl_req = cl_set ? (uint32_t)strtoul(cl_env, nullptr, 10) : (uint32_t)kStCluster;
+    if (cl_req != 0u && cl_req != (uint32_t)kStCluster) return fail(NB200_EINVAL, "NB200_STREAM_CLUSTER=%s: 0 or %d", cl_env, kStCluster);
+    uint32_t chunk_target = 32768u / (d.hd * 8u); chunk_target &= ~7u; if (chunk_target < 32) chunk_target = 32;      // measured: ~32 KB of K+V per (kv head, split) item
+    chunk_target = env_u32("NB200_ATTN_CHUNK", chunk_target);
+    if (chunk_target < 8) chunk_target = 8;
+    StreamKern kcl = nullptr;
+    {
+        const uint32_t ns = st_splits_max(d, chunk_target, nsplit_max);
+        if (cl_req && ns <= (uint32_t)kStCluster && d.KV * (uint32_t)kStCluster <= NC) kcl = pick_stream(d, true);
+        if (cl_set && cl_req && !kcl) return fail(NB200_EINVAL, "NB200_STREAM_CLUSTER=%s: this model at %u positions has %u splits per kv head, "
+                                                  "%u kv heads: the cluster launch takes at most %d splits and %u kv heads", cl_env, d.max_seq, ns, d.KV, kStCluster, NC / kStCluster);
+    }
 
     StreamArgs &g = e->sa;
     memset(&g, 0, sizeof g);
@@ -808,14 +865,20 @@ int setup_stream(nb200_engine *e) {
     // phase never waits for the slowest warp of the previous one before it writes its operand.  The ring stage is 16 KB by default and
     // shrinks in 1 KB steps (never below one row unit of the longest row) until kStSegTiles + 4 stages fit beside the fixed regions.
     auto al = [](uint32_t v) { return (v + 127u) & ~127u; };
-    const uint32_t nsplit_max = e->nsplit_max;          // num_sms / kv heads (<= 64), as the multi-kernel path
     const uint32_t act_b = al(act_region_bytes(d.quant, maxn, d.gs ? d.gs : 1));
     g.off_act = 0; g.off_act2 = act_b; g.off_xs = 2 * act_b; g.off_attn = g.off_xs + al(d.E * 4u);
     int max_optin = 0;
     CK(cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->device));
     cudaFuncAttributes fattr;
     CK(cudaFuncGetAttributes(&fattr, (const void *)k));
-    const uint32_t static_smem = al((uint32_t)fattr.sharedSizeBytes);   // mbarriers, row ranges, residual rows, reduction scratch
+    uint32_t static_smem = al((uint32_t)fattr.sharedSizeBytes);   // mbarriers, row ranges, residual rows, reduction scratch
+    if (kcl) {
+        CK(cudaFuncGetAttributes(&fattr, (const void *)kcl));
+        if (al((uint32_t)fattr.sharedSizeBytes) > static_smem) static_smem = al((uint32_t)fattr.sharedSizeBytes);
+    }
+    // cluster launch: split 0's merge staging follows the attention workspace (16-byte mbarrier + phase count, then floats); the
+    // plain launch's staging overlays the workspace instead, so the two plans share one region: the larger of the two
+    const uint32_t rx_b = kcl ? al(16u + st_attn_rx_floats(d.kv_mul, d.hd, nsplit_max) * 4u) : 0u;
     const uint32_t min_stage = (unit_b_max + 16u + 1023u) & ~1023u;
     uint32_t stage_bytes = env_u32("NB200_STAGE_KB", 16) * 1024u;
     if (stage_bytes < min_stage) stage_bytes = min_stage;
@@ -824,7 +887,9 @@ int setup_stream(nb200_engine *e) {
     for (;; stage_bytes -= 1024u) {
         kv_rows = (stage_bytes / (2u * d.hd * 4u)) & ~3u;
         if (kv_rows < 4) return 0;
-        const uint32_t attn_b = al(st_attn_smem_floats(d.kv_mul, d.hd, nsplit_max, (uint32_t)kStSegTiles * kv_rows) * 4u);
+        uint32_t attn_b = al(st_attn_smem_floats(d.kv_mul, d.hd, nsplit_max, (uint32_t)kStSegTiles * kv_rows) * 4u);
+        const uint32_t attn_cl_b = kcl ? al(st_attn_work_floats(d.kv_mul, d.hd, (uint32_t)kStSegTiles * kv_rows) * 4u) + rx_b : 0u;
+        if (attn_cl_b > attn_b) attn_b = attn_cl_b;
         region0 = g.off_attn + attn_b;
         nst = (uint32_t)max_optin > static_smem + region0 ? ((uint32_t)max_optin - static_smem - region0) / stage_bytes : 0u;
         if (nst > nst_cap) nst = nst_cap;
@@ -832,6 +897,7 @@ int setup_stream(nb200_engine *e) {
         if (stage_bytes < min_stage + 1024u) return 0;
     }
     g.off_ring = region0;
+    g.off_rx = kcl ? g.off_attn + al(st_attn_work_floats(d.kv_mul, d.hd, (uint32_t)kStSegTiles * kv_rows) * 4u) : 0u;
     for (int i = 0; i < 5; i++) {                       // a stage holds one row unit of every kind (tiles: st_layout)
         const StKind &sk = g.kind[i];
         const uint32_t T = (stage_bytes - 16u) / (sk.row_stride + sk.aux_stride);
@@ -843,6 +909,25 @@ int setup_stream(nb200_engine *e) {
     int occ = 0;
     if (ce == cudaSuccess) ce = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (const void *)k, kThreads, smem);
     if (ce != cudaSuccess || occ < 1) { cudaGetLastError(); return 0; }
+    e->st_max_clusters = 0;
+    if (kcl) {          // clusters of kStCluster CTAs that are resident at once (0: the cluster launch is not used)
+        ce = cudaFuncSetAttribute((const void *)kcl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        int ncl = 0;
+        if (ce == cudaSuccess) {
+            cudaLaunchConfig_t cfg = {};
+            cfg.gridDim = dim3(kStCluster); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem;
+            cudaLaunchAttribute attr[1];
+            attr[0].id = cudaLaunchAttributeClusterDimension;
+            attr[0].val.clusterDim.x = kStCluster; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+            cfg.attrs = attr; cfg.numAttrs = 1;
+            ce = cudaOccupancyMaxActiveClusters(&ncl, (const void *)kcl, &cfg);
+        }
+        if (ce != cudaSuccess) { cudaGetLastError(); ncl = 0; }
+        if ((uint32_t)ncl >= d.KV) e->st_max_clusters = (uint32_t)ncl;
+        if (cl_set && !e->st_max_clusters)
+            return fail(NB200_EINVAL, "NB200_STREAM_CLUSTER=%s: %d clusters of %d CTAs are resident at once, this model needs %u", cl_env, ncl, kStCluster, d.KV);
+    }
+    e->st_cl_forced = cl_set && cl_req;
 
     if (!e->bar) { DM(e->bar, 64); CK(cudaMemset(e->bar, 0, 64)); }
     CK(cudaHostAlloc(&e->st_err_host, 64, cudaHostAllocMapped));
@@ -869,14 +954,17 @@ int setup_stream(nb200_engine *e) {
     g.cls_val = e->cls_val; g.cls_idx = e->cls_idx;
     g.st = e->st; g.ids = e->ids_dev; g.seen = e->seen; g.bar = e->bar; g.err = e->st_err_dev;
     g.n_steps = 1; g.nsplit_max = nsplit_max;
-    uint32_t ct = 32768u / (d.hd * 8u); ct &= ~7u; if (ct < 32) ct = 32;      // measured: ~32 KB of K+V per (kv head, split) item
-    g.chunk_target = env_u32("NB200_ATTN_CHUNK", ct);
+    g.chunk_target = chunk_target;
     g.ablate = env_u32("NB200_ABLATE", 0);
-    if (g.chunk_target < 8) g.chunk_target = 8;
     g.d = d;
 
-    // NB200_STREAM_WIDTH=<W> fixes the grid width (tests, sweeps); otherwise calibrate_width picks it after creation
+    // NB200_STREAM_WIDTH=<W> fixes the grid width (tests, sweeps); otherwise calibrate_width picks it after creation, starting
+    // from num_sms, or the widest cluster launch where that is allowed
     uint32_t W = NC;
+    if (e->st_max_clusters) {
+        const uint32_t wc = (NC / kStCluster < e->st_max_clusters ? NC / kStCluster : e->st_max_clusters) * (uint32_t)kStCluster;
+        if (st_cl_width_ok(e, wc)) W = wc;
+    }
     const char *wenv = getenv("NB200_STREAM_WIDTH");
     if (wenv && *wenv) {
         W = (uint32_t)strtoul(wenv, nullptr, 10);
@@ -884,8 +972,9 @@ int setup_stream(nb200_engine *e) {
         if (W < wmin || W > NC) return fail(NB200_EINVAL, "NB200_STREAM_WIDTH=%s: this model's streaming kernel runs on %u..%u CTAs", wenv, wmin, NC);
         e->st_width_fixed = true;
     }
+    e->st_kern_plain = (const void *)k; e->st_kern_cl = (const void *)kcl;
     if ((r = st_layout(e, W))) return r;
-    e->st_kern = (const void *)k; e->st_smem = smem; e->use_stream = true; e->launches_per_token = 1;
+    e->st_smem = smem; e->use_stream = true; e->launches_per_token = 1;
     return 0;
 }
 
@@ -1277,17 +1366,28 @@ static int calibrate_paths(nb200_engine *e) {
 // st_width_min).  A narrower grid has fewer CTAs to exchange with and wait for in every phase, and more rows per CTA; where a
 // phase's rows per CTA outgrow one ring tile, the time steps up (DESIGN.md section 5.4: Nano-168M Q80 is fastest from 110 to
 // 128 CTAs of 132).  Each width needs its own stream copy of the weights (st_layout), built in place.
+// Where the cluster launch is allowed, only its legal widths are timed: the same fractions rounded down to a multiple of
+// kStCluster and within the resident clusters (st_cl_width_ok; Nano-168M Q80 on an H100 with 14 resident clusters of 8: 112, 96, 64).
 static int calibrate_width(nb200_engine *e) {
     const uint32_t n = 8;
     const uint32_t lim = pos_limit(e->d);
     const uint32_t NS = (uint32_t)e->num_sms, wmin = st_width_min(e);
-    const uint32_t cand[6] = {NS, (15 * NS) / 16, (7 * NS) / 8, (3 * NS) / 4, NS / 2, NS / 3};
+    uint32_t cand[6] = {NS, (15 * NS) / 16, (7 * NS) / 8, (3 * NS) / 4, NS / 2, NS / 3};
+    const bool cl = e->st_cl != 0u;
+    if (cl) {
+        for (uint32_t &W : cand) {
+            W -= W % (uint32_t)kStCluster;
+            if (W / kStCluster > e->st_max_clusters) W = e->st_max_clusters * (uint32_t)kStCluster;
+        }
+    }
     if (lim < 4 * n || cand[1] < wmin) return 0;
     uint32_t best_w = e->st_grid;
     float best = 0.0f;
     int r;
-    for (uint32_t W : cand) {
+    for (int i = 0; i < 6; i++) {
+        const uint32_t W = cand[i];
         if (W < wmin) break;
+        if (cl && ((i > 0 && W == cand[i - 1]) || !st_cl_width_ok(e, W))) continue;
         if (W != e->st_grid && (r = st_layout(e, W))) return r;
         float ms = 0.0f;
         if ((r = time_steps(e, lim / 2, n, ms))) return r;
@@ -1432,7 +1532,8 @@ int nb200_get_config(const nb200_engine *e, nb200_config *c) {
     c->block_size = d.block_size; c->vocab_size = d.V; c->n_layer = d.L; c->n_embd = d.E;
     c->n_head = e->g_H; c->n_kv_head = e->g_KV; c->n_hidden = d.F; c->tied = e->tied ? 1u : 0u; c->head_dim = d.hd;
     c->q_dim = e->g_q_dim; c->kv_dim = e->g_kv_dim; c->max_seq_len = d.max_seq; c->tp_rank = e->tp_rank; c->tp_size = e->tp_size;
-    c->reserved[0] = e->use_stream ? 4u | e->st_grid << 8 : (e->graph ? 1u : 0u);    // execution path: 4 | CTAs << 8 streaming kernel, 1 graph, 0 direct launches
+    // execution path: 4 | CTAs << 8 | CTAs per cluster << 24 streaming kernel (0 per cluster: plain launch), 1 graph, 0 direct launches
+    c->reserved[0] = e->use_stream ? 4u | e->st_grid << 8 | e->st_cl << 24 : (e->graph ? 1u : 0u);
     c->reserved[1] = (uint32_t)(e->calib_ms[0] * 1000.0f + 0.5f);     // calibrate_paths: microseconds per token of the streaming kernel ...
     c->reserved[2] = (uint32_t)(e->calib_ms[1] * 1000.0f + 0.5f);     // ... and of the multi-kernel graph (0 = the choice was not measured)
     c->reserved[3] = e->mv_mask;

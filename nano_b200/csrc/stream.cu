@@ -1,5 +1,6 @@
-// stream.cu -- translation unit of the grid-wide streaming decode kernel (stream.cuh): kernel instantiations + the
-// load-time builder of the per-CTA weight streams.  Compiled beside engine.cu so the two build in parallel.
+// stream.cu -- translation unit of the grid-wide streaming decode kernel (stream.cuh): the plain launch's kernel instantiations
+// + the load-time builder of the per-CTA weight streams.  Compiled beside engine.cu and stream_cl.cu (the cluster launch's
+// instantiations) so that they build in parallel.
 #define NB_K static
 #include "stream_host.h"
 #include "stream.cuh"
@@ -34,23 +35,9 @@ cudaError_t stream_build_launch(const uint8_t *mainp, const uint8_t *auxp, uint3
     return cudaGetLastError();
 }
 
-template <int QUANT, int LPG>
-static StreamKern pick_stream_kvm(uint32_t kvm) {
-    switch (kvm) {
-        case 1: return k_decode_stream<QUANT, LPG, 1>;
-        case 2: return k_decode_stream<QUANT, LPG, 2>;
-        case 4: return k_decode_stream<QUANT, LPG, 4>;
-        default: return nullptr;
-    }
-}
-
-StreamKern pick_stream(const Dims &d) {
+StreamKern pick_stream(const Dims &d, bool cluster) {
     if (d.hd > 128 || (d.arch == 3u && (d.hd & (d.hd - 1)) != 0)) return nullptr;     // in-register half-split RoPE needs hd = 4 * 2^k
-    if (d.quant == 0x00u) return pick_stream_kvm<0x00, 8>(d.kv_mul);
-    if (d.quant == 0x42u) return pick_stream_kvm<0x42, 8>(d.kv_mul);
-    if (d.gs == 128) return pick_stream_kvm<0x80, 8>(d.kv_mul);
-    if (d.gs == 64) return pick_stream_kvm<0x80, 4>(d.kv_mul);
-    return nullptr;
+    return cluster ? pick_stream_cluster(d) : st_pick<0>(d);
 }
 
 }  // namespace nb

@@ -28,6 +28,7 @@
 #pragma once
 #include "kernels.cuh"
 #include "stream_args.h"
+#include "stream_host.h"
 
 namespace nb {
 
@@ -71,6 +72,32 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity, uint32
         if (sleep_ns) __nanosleep(sleep_ns);
         if (clock64() - t0 > 4000000000ll) st_give_up(err, code);
     }
+}
+// ---- distributed shared memory (cluster launch only): split s of a kv head hands its partial to split 0's CTA
+// the address of the same shared-memory byte in the CTA of cluster rank `rank`
+__device__ __forceinline__ uint32_t dsm_map(uint32_t a, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
+    return r;
+}
+// one word into another CTA's shared memory; its 4 bytes complete_tx on that CTA's mbarrier (both cluster addresses)
+__device__ __forceinline__ void dsm_st_async(uint32_t a, float v, uint32_t bar) {
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(a), "r"(__float_as_uint(v)), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// mbar_wait for bytes that other CTAs of the cluster wrote (acquire at cluster scope)
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t *bar, uint32_t parity, uint32_t *err, uint32_t code) {
+    auto ok = [&]() -> bool {
+        uint32_t v;
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(v) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+        return v != 0;
+    };
+    if (ok()) return;
+    const long long t0 = clock64();
+    while (!ok()) { if (clock64() - t0 > 4000000000ll) st_give_up(err, code); }
 }
 // threadIdx.x through an opaque read, in the consumers' device functions: the compiler cannot hoist what is derived from it
 // (lane offsets, slot indices) out of the layer loop, where it would stay live across every phase (128-register cap)
@@ -182,6 +209,19 @@ __device__ __forceinline__ void st_attn_plan(uint32_t range, uint32_t nsplit_max
     chunk = c;
     nsplit = (range + c - 1) / c;
 }
+// The attention item (kv head, split) CTA `cta` runs, false if none; the producer and the consumers both ask here.
+//   plain launch (CL = 0): CTA i runs item i = kvh * nsplit + sp;
+//   cluster launch of CL CTAs per cluster (nsplit <= CL): cluster h runs kv head h, its CTA of rank sp split sp.
+template <int CL>
+__device__ __forceinline__ bool st_item(uint32_t cta, uint32_t KV, uint32_t nsplit, uint32_t &kvh, uint32_t &sp) {
+    if constexpr (CL > 0) {
+        kvh = cta / (uint32_t)CL; sp = cta % (uint32_t)CL;
+        return kvh < KV && sp < nsplit;
+    } else {
+        kvh = cta / nsplit; sp = cta % nsplit;
+        return cta < KV * nsplit;
+    }
+}
 
 struct StRing {
     uint64_t *full, *empty;
@@ -224,6 +264,7 @@ __device__ __forceinline__ void st_issue_kind(const StreamArgs &g, const StRing 
     }
 }
 
+template <int CL>
 static __device__ void st_producer(const StreamArgs &g, const StRing &r, const StOwn &own, uint32_t cta, volatile uint32_t *progress,
                                    uint32_t pos0, uint32_t causal, uint32_t advance) {
     const Dims &d = g.d;
@@ -239,8 +280,8 @@ static __device__ void st_producer(const StreamArgs &g, const StRing &r, const S
         for (uint32_t l = 0; l < d.L; l++) {
             const uint8_t *lb = base + (uint64_t)l * g.layer_stride;
             st_issue_kind(g, r, c, issued, g.kind[SK_QKV], lb, own.rows[SK_QKV]);
-            if (cta < d.KV * nsplit) {
-                const uint32_t kvh = cta / nsplit, sp = cta % nsplit;
+            uint32_t kvh, sp;
+            if (st_item<CL>(cta, d.KV, nsplit, kvh, sp)) {
                 const uint32_t t0 = min(range, sp * chunk), t1 = min(range, t0 + chunk);
                 const float *kb = g.kc + l * kvl + (size_t)kvh * d.max_seq * d.hd;
                 const float *vb = g.vc + l * kvl + (size_t)kvh * d.max_seq * d.hd;
@@ -803,14 +844,14 @@ __device__ __forceinline__ void st_consume(const StreamArgs &g, const StRing &r,
 // rows (this step's QKV outputs) are written into their slots of the resident tile, so the passes treat all rows alike.
 // A range held by one item is normalised and published at once; otherwise every item publishes its partial and the item
 // of split 0 merges them in split order.
-template <int KVM>
+template <int KVM, int CL>
 static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCursor &c, uint32_t &tcount, uint32_t layer, uint32_t cta, uint32_t pos, uint32_t range,
                                     uint32_t nsplit, uint32_t chunk, uint32_t e_in, uint32_t e_out, float *sm, unsigned long long *dbg) {
     const Dims &d = g.d;
-    if (cta >= d.KV * nsplit) return;
+    uint32_t kvh, sp;
+    if (!st_item<CL>(cta, d.KV, nsplit, kvh, sp)) return;
     ST_DBG(0);
     const uint32_t hd = d.hd, hd4 = hd / 4u, hd2 = hd / 2u;
-    const uint32_t kvh = cta / nsplit, sp = cta % nsplit;
     const uint32_t t0 = min(range, sp * chunk), t1 = min(range, t0 + chunk);
     const size_t kvl = (size_t)d.KV * d.max_seq * hd;
     float *kbase = g.kc + layer * kvl + (size_t)kvh * d.max_seq * hd;
@@ -995,41 +1036,68 @@ static __device__ void st_attention(const StreamArgs &g, const StRing &r, StCurs
         return;
     }
     unsigned long long *part = g.xws + ((size_t)kvh * g.nsplit_max) * pw;
-    if (sp != 0) {              // publish the partial; split 0 of the kv head merges
-        for (uint32_t idx = st_tid(); idx < pw; idx += kConsThreads) xw_st(part + (size_t)sp * pw + idx, outp[idx], e_out);
-        return;
-    }
-    ST_DBG(9);
-    // ---- merge (split 0): own partial from shared memory, the others polled from the exchange words ----
+    // Merge staging of split 0: the partials of all splits, [KVM][nsplit][hd] accumulators, then the maxima / merge weights
+    // [KVM][nsplit_max], the totals [KVM] and the partial sums [KVM][nsplit_max].  Plain launch: over this CTA's own work area
+    // (free once its partial is in registers).  Cluster launch: in a region of its own (st_attn_rx_floats) behind an mbarrier,
+    // which the other splits fill through distributed shared memory while split 0 may still be attending.
     uint32_t region = st_attn_work_floats(KVM, hd, seg_max);
-    if (g.nsplit_max * KVM * hd > region) region = g.nsplit_max * KVM * hd;
-    float *wsc = sm + region;                            // [KVM][nsplit_max] weights e^{m_s - M}; before that: the maxima
-    float *stat = wsc + KVM * g.nsplit_max;              // [KVM] L, then [KVM][nsplit_max] partial sums
-    float own[4];                                        // this thread's slice of the own partial (pw <= 4 * 480 for hd <= 128, KVM <= 8)
-#pragma unroll
-    for (int u = 0; u < 4; u++) { const uint32_t idx = st_tid() + u * kConsThreads; own[u] = idx < pw ? outp[idx] : 0.0f; }
-    cbar();                                              // outp / ws are about to be overwritten by the staging area
-    float *macc = sm;                                    // [KVM][nsplit][hd]
-    float *pl = stat + KVM;                              // [KVM][nsplit_max]
-    auto place = [&](uint32_t s2, uint32_t idx, float v) {
-        const uint32_t m = idx / (hd + 2), i = idx % (hd + 2);
-        if (i < hd) macc[(m * nsplit + s2) * hd + i] = v;
-        else if (i == hd) wsc[m * g.nsplit_max + s2] = v;
-        else pl[m * g.nsplit_max + s2] = v;
-    };
-#pragma unroll
-    for (int u = 0; u < 4; u++) { const uint32_t idx = st_tid() + u * kConsThreads; if (idx < pw) place(0, idx, own[u]); }
-    for (uint32_t e0 = pw + st_tid(); e0 < nsplit * pw; e0 += 8u * kConsThreads) {       // eight loads in flight per thread before any epoch is checked
-        unsigned long long w8[8];
-#pragma unroll
-        for (int u = 0; u < 8; u++) { const uint32_t e = e0 + u * kConsThreads; if (e < nsplit * pw) w8[u] = xw_ld1(part + e); }
-#pragma unroll
-        for (int u = 0; u < 8; u++) {
-            const uint32_t e = e0 + u * kConsThreads;
-            if (e < nsplit * pw) place(e / pw, e % pw, xw_ok(w8[u], e_out) ? xw_val(w8[u]) : xw_poll1(part + e, e_out, g.err));
-        }
+    float *macc;
+    if constexpr (CL > 0) {
+        macc = reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(sm) - g.off_attn + g.off_rx + 16u);
+    } else {
+        macc = sm;
+        if (g.nsplit_max * KVM * hd > region) region = g.nsplit_max * KVM * hd;
     }
-    cbar();
+    float *wsc = (CL > 0) ? macc + KVM * (uint32_t)CL * hd : sm + region;      // [KVM][nsplit_max] weights e^{m_s - M}; before that: the maxima
+    float *stat = wsc + KVM * g.nsplit_max;              // [KVM] L, then [KVM][nsplit_max] partial sums
+    float *pl = stat + KVM;                              // [KVM][nsplit_max]
+    auto slot = [&](uint32_t s2, uint32_t idx) -> float * {
+        const uint32_t m = idx / (hd + 2), i = idx % (hd + 2);
+        if (i < hd) return macc + (m * nsplit + s2) * hd + i;
+        else if (i == hd) return wsc + m * g.nsplit_max + s2;
+        else return pl + m * g.nsplit_max + s2;
+    };
+    if constexpr (CL > 0) {
+        uint64_t *rxbar = reinterpret_cast<uint64_t *>(reinterpret_cast<unsigned char *>(sm) - g.off_attn + g.off_rx);
+        if (sp != 0) {          // the partial into split 0's staging, each word where split 0 would place it
+            const uint32_t bar0 = dsm_map(smem_u32(rxbar), 0u);
+            for (uint32_t idx = st_tid(); idx < pw; idx += kConsThreads) dsm_st_async(dsm_map(smem_u32(slot(sp, idx)), 0u), outp[idx], bar0);
+            return;
+        }
+        ST_DBG(9);
+        // ---- merge (split 0): own partial from shared memory, the others' words arrive on the local mbarrier ----
+        volatile uint32_t *rxn = reinterpret_cast<volatile uint32_t *>(rxbar + 1);      // merges completed so far: the phase parity
+        const uint32_t par = *rxn & 1u;
+        for (uint32_t idx = st_tid(); idx < pw; idx += kConsThreads) *slot(0, idx) = outp[idx];
+        if (st_tid() == 0) mbar_expect_tx(rxbar, (nsplit - 1u) * pw * 4u);
+        mbar_wait_cluster(rxbar, par, g.err, 0x32u);
+        cbar();
+        if (st_tid() == 0) *rxn = *rxn + 1u;             // every thread has read the parity (before the barrier above)
+    } else {
+        if (sp != 0) {          // publish the partial; split 0 of the kv head merges
+            for (uint32_t idx = st_tid(); idx < pw; idx += kConsThreads) xw_st(part + (size_t)sp * pw + idx, outp[idx], e_out);
+            return;
+        }
+        ST_DBG(9);
+        // ---- merge (split 0): own partial from shared memory, the others polled from the exchange words ----
+        float own[4];                                        // this thread's slice of the own partial (pw <= 4 * 480 for hd <= 128, KVM <= 8)
+#pragma unroll
+        for (int u = 0; u < 4; u++) { const uint32_t idx = st_tid() + u * kConsThreads; own[u] = idx < pw ? outp[idx] : 0.0f; }
+        cbar();                                              // outp / ws are about to be overwritten by the staging area
+#pragma unroll
+        for (int u = 0; u < 4; u++) { const uint32_t idx = st_tid() + u * kConsThreads; if (idx < pw) *slot(0, idx) = own[u]; }
+        for (uint32_t e0 = pw + st_tid(); e0 < nsplit * pw; e0 += 8u * kConsThreads) {       // eight loads in flight per thread before any epoch is checked
+            unsigned long long w8[8];
+#pragma unroll
+            for (int u = 0; u < 8; u++) { const uint32_t e = e0 + u * kConsThreads; if (e < nsplit * pw) w8[u] = xw_ld1(part + e); }
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+                const uint32_t e = e0 + u * kConsThreads;
+                if (e < nsplit * pw) *slot(e / pw, e % pw) = xw_ok(w8[u], e_out) ? xw_val(w8[u]) : xw_poll1(part + e, e_out, g.err);
+            }
+        }
+        cbar();
+    }
     ST_DBG(10);
     if (warp < KVM) {
         float pm[2], pls[2];                             // nsplit_max <= 64: two slots per lane
@@ -1080,7 +1148,9 @@ __device__ __forceinline__ void st_grid_barrier(const StreamArgs &g, unsigned in
 }
 
 // ---------------------------------------------------------------- the kernel
-template <int QUANT, int LPG, int KVM>
+// CL > 0: launched in clusters of CL CTAs (st_item), the split partials of a kv head travel to split 0 through distributed
+// shared memory (st_attention); CL = 0: a plain cooperative launch
+template <int QUANT, int LPG, int KVM, int CL>
 __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_constant__ StreamArgs gparam) {
     extern __shared__ __align__(128) unsigned char ssm[];
     // The argument block is read from shared memory: kernel parameters live in the constant bank, whose cache shares the
@@ -1114,6 +1184,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
         ss.causal = __ldcg(&g.st->is_causal); ss.n_prompt = __ldcg(&g.st->n_prompt); ss.advance = __ldcg(&g.st->advance);
         ss.pen = __ldcg(&g.st->penalty);
         ss.tok = __ldcg(&g.st->use_token) ? __ldcg(&g.st->token) : __ldcg(g.ids + ss.pos);
+        if (CL > 0) {           // the merge staging's mbarrier (st_attention) and its phase count
+            uint64_t *rxbar = reinterpret_cast<uint64_t *>(ssm + g.off_rx);
+            mbar_init(rxbar, 1);
+            *reinterpret_cast<volatile uint32_t *>(rxbar + 1) = 0u;
+        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (uint32_t i = threadIdx.x; i < 2u * kStGroupsMax; i += kThreads) s_ready[i / kStGroupsMax][i % kStGroupsMax] = 0u;
@@ -1150,9 +1225,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
         geo.gl[kid][ln] = (uint8_t)(tl / lg2); geo.ul[kid][ln] = (uint8_t)(tl % lg2);
     }
     __syncthreads();
+    if constexpr (CL > 0) cluster_sync_all();      // no partial is sent before split 0's mbarrier is initialised
 
     if (warp == kConsWarps) {
-        if (lane == 0) st_producer(g, ring_of(), own, cta, &s_progress, ss.pos, ss.causal, ss.advance);
+        if (lane == 0) st_producer<CL>(g, ring_of(), own, cta, &s_progress, ss.pos, ss.causal, ss.advance);
         return;
     }
 
@@ -1172,6 +1248,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
         if (st_tid() == 0) {       // read by the others after the barrier below
             ss.range = ss.causal ? ss.pos + 1u : d.max_seq;
             st_attn_plan(ss.range, g.nsplit_max, g.chunk_target, ss.nsplit, ss.chunk);
+            // cluster launch: a kv head's splits are the ranks of one cluster (the host admits only shapes where they fit)
+            if (CL > 0 && ss.nsplit > (uint32_t)CL) st_give_up(g.err, 0x33u);
         }
         // embedding row (infer.c:987-988) into shared memory; the rows this CTA owns in the residual phases start from it
         {
@@ -1228,7 +1306,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
                 ST_TRACE();
                 if (cls) break;
                 if (ph == SK_QKV) {
-                    st_attention<KVM>(g, ring_of(), cur, tcount, l, cta, ss.pos, ss.range, ss.nsplit, ss.chunk, (g.ablate & 16u) ? kXwAny : el + 1u, el + 2u, reinterpret_cast<float *>(ssm + g.off_attn), dbg ? g.trace + 1100 + 64 : nullptr);
+                    st_attention<KVM, CL>(g, ring_of(), cur, tcount, l, cta, ss.pos, ss.range, ss.nsplit, ss.chunk, (g.ablate & 16u) ? kXwAny : el + 1u, el + 2u, reinterpret_cast<float *>(ssm + g.off_attn), dbg ? g.trace + 1100 + 64 : nullptr);
                     ST_STAMP();
                     ST_TRACE();
                 }
@@ -1286,6 +1364,26 @@ __global__ void __launch_bounds__(kThreads, 1) k_decode_stream(const __grid_cons
     }
 #undef ST_TRACE
 #undef ST_STAMP
+}
+
+// the instantiation for a model shape: stream.cu instantiates the plain launch's (CL = 0), stream_cl.cu the cluster launch's
+template <int QUANT, int LPG, int CL>
+static StreamKern st_pick_kvm(uint32_t kvm) {
+    switch (kvm) {
+        case 1: return k_decode_stream<QUANT, LPG, 1, CL>;
+        case 2: return k_decode_stream<QUANT, LPG, 2, CL>;
+        case 4: return k_decode_stream<QUANT, LPG, 4, CL>;
+        default: return nullptr;
+    }
+}
+
+template <int CL>
+static StreamKern st_pick(const Dims &d) {
+    if (d.quant == 0x00u) return st_pick_kvm<0x00, 8, CL>(d.kv_mul);
+    if (d.quant == 0x42u) return st_pick_kvm<0x42, 8, CL>(d.kv_mul);
+    if (d.gs == 128) return st_pick_kvm<0x80, 8, CL>(d.kv_mul);
+    if (d.gs == 64) return st_pick_kvm<0x80, 4, CL>(d.kv_mul);
+    return nullptr;
 }
 
 }  // namespace nb

@@ -10,6 +10,7 @@ constexpr int kConsThreads = kConsWarps * 32;
 constexpr int kStMaxStages = 24;
 constexpr int kStRep = 8;                         // replicas of every activation vector that ALL CTAs read (spread over L2 slices)
 constexpr int kStOwnMax = 128;                    // residual rows one CTA can own (n_embd <= 128 * CTAs)
+constexpr int kStCluster = 8;                     // CTAs per cluster of the cluster launch (the portable maximum): one kv head, at most 8 splits
 enum { EPI_ATTN = 5 };
 enum StKindId { SK_QKV = 0, SK_O = 1, SK_W13 = 2, SK_W2 = 3, SK_CLS = 4 };
 
@@ -30,6 +31,7 @@ struct StreamArgs {
     StKind kind[5];
     uint32_t nstages, stage_bytes, kv_tile_rows, kv_tile_magic;      // magic = ceil(2^32 / kv_tile_rows): idx / kv_tile_rows == umulhi(idx, magic) for idx < 65536
     uint32_t off_ring, off_act, off_act2, off_xs, off_attn;     // byte offsets inside dynamic shared memory (two activation operands: consecutive phases alternate)
+    uint32_t off_rx;                                  // cluster launch: split 0's merge staging (mbarrier, phase count, st_attn_rx_floats); 0 otherwise
     const float *g_attn, *g_ffn, *g_final;            // rmsnorm gains [L][E], [L][E], [E]
     const float *qnorm, *knorm, *rope_cos, *rope_sin;
     const void *emb_w, *emb_aux;
@@ -73,6 +75,12 @@ __host__ __device__ inline uint32_t st_attn_smem_floats(uint32_t kvm, uint32_t h
     const uint32_t merge = nsplit_max * kvm * hd;
     if (merge > ws) ws = merge;
     return ws + 2u * kvm * nsplit_max + 2u * kvm + 16u;
+}
+// cluster launch: split 0's merge staging, a region of its own right behind the workspace st_attn_work_floats (which it does
+// not overlay, unlike the plain launch's staging), floats after a 16-byte mbarrier + phase count:
+// accumulators [KVM][kStCluster][hd], maxima / weights [KVM][nsplit_max], totals [KVM], partial sums [KVM][nsplit_max]
+__host__ __device__ inline uint32_t st_attn_rx_floats(uint32_t kvm, uint32_t hd, uint32_t nsplit_max) {
+    return kvm * (uint32_t)kStCluster * hd + 2u * kvm * nsplit_max + kvm;
 }
 
 }  // namespace nb

@@ -162,10 +162,12 @@ class Engine:
         self.path = {4: "streaming kernel (persistent grid, per-CTA TMA ring over weights and KV, L2 grid barriers)",
                      1: "multi-kernel CUDA graph with PDL", 0: "multi-kernel direct launches"}[int(cfg.reserved[0]) & 0xff]
         # streaming kernel: CTAs of its grid (NB200_STREAM_WIDTH, or the fastest width timed at creation); None on the other paths
-        self.stream_width = (int(cfg.reserved[0]) >> 8) or None
+        self.stream_width = ((int(cfg.reserved[0]) >> 8) & 0xffff) or None
+        # CTAs per thread-block cluster of the streaming kernel's launch; None on a plain launch and on the other paths
+        self.stream_cluster = (int(cfg.reserved[0]) >> 24) or None
         # creation-time calibration of the two fast paths (large one-GPU Q80 engines): us per token of each, None when not measured
         self.calibration = ({"streaming_us_per_token": int(cfg.reserved[1]), "multikernel_us_per_token": int(cfg.reserved[2]),
-                             "stream_width": self.stream_width}
+                             "stream_width": self.stream_width, "stream_cluster": self.stream_cluster}
                             if int(cfg.reserved[1]) and int(cfg.reserved[2]) else None)
 
     def kernels(self) -> dict:
